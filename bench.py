@@ -31,7 +31,7 @@ WORKLOADS = {   # name -> (task, num_envs per GPU, algorithmic bytes per env-ste
     "anymal": ("AnymalTerrain", 4096, 2250),
     "shadow_hand": ("ShadowHand", 4096, 3640),    # BASELINE.json config 5: 32768 envs over 8 GPUs
 }
-METRIC = "env-steps/s at num_envs=16384 (Ant), 1/2/4/8 B200; %HBM roofline"
+METRIC = "env-steps/s at num_envs=16384 (Ant), 1/2/4/8 H100; %HBM roofline"
 PARITY_NOTE = ("obs/reward/reset arithmetic pinned by the reference's own functions; physics parity UNPINNED against PhysX "
                "(closed gym.simulate): engine == own fp64 oracle only")
 
@@ -41,11 +41,11 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback"              # H100 SXM data sheet, HBM3
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -342,6 +342,27 @@ def run_reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------ GPU arm
+DUMP_LIMIT = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, step_result):
+    """What the last timed VecTask.step() returned -- obs dict, reward, reset, time_outs -- as <out_dir>/<name>.npy (float32).
+    An array that would take the total over DUMP_LIMIT is reduced to a fixed, seeded sample of its rows (indices saved beside it)."""
+    obs, rew, reset, extras = step_result
+    arrays = {f"obs_{k}": v for k, v in obs.items()}
+    arrays.update(rew=rew, reset=reset, time_outs=extras["time_outs"])
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT
+    for name, t in sorted(arrays.items()):
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget // 2:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=max(1, a.shape[0] * (budget // 2) // a.nbytes), replace=False))
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        budget -= a.nbytes
+
+
 def run_gpu_arm(args):
     import torch
     import torch.distributed as dist
@@ -360,7 +381,7 @@ def run_gpu_arm(args):
     # L2-resident between steps, so the bench steps R independent env sets round-robin with R * n * bytes_per >= 1.5 x L2:
     # by the time a set is stepped again, everything it reads has been evicted and comes from HBM, while the kernel's
     # code stays warm, as in a real rollout loop.
-    L2_BYTES = 126 * 1024 * 1024
+    L2_BYTES = 50 * 1024 * 1024                         # H100
     R = args.sets if args.sets > 0 else max(2, -(-int(1.5 * L2_BYTES) // (n * bytes_per)))
     R = min(R, 192)
     envs = [make_env(task, n, device, rank) for _ in range(R)]
@@ -368,7 +389,7 @@ def run_gpu_arm(args):
     A = env.num_actions
     gen = torch.Generator(device=device).manual_seed(42 + rank)
     ring = [2 * torch.rand((n, A), device=device, generator=gen) - 1 for _ in range(16)]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=device)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=device)   # > 50 MB L2
 
     def barrier():
         D.barrier()
@@ -386,10 +407,12 @@ def run_gpu_arm(args):
     w0 = time.perf_counter()
     t0.record()
     for k in range(args.steps):
-        envs[k % R].step(ring[k % 16])
+        last = envs[k % R].step(ring[k % 16])
     t1.record()
     host_issue_s = time.perf_counter() - w0                 # host time to ISSUE the K steps (no sync inside)
     barrier()
+    if args.dump_outputs and rank == 0:                     # before later legs step the same env set again
+        dump_outputs(args.dump_outputs, last)
     launches = sum(e_.sim.launch_count() for e_ in envs) - l0
     total_ms = t0.elapsed_time(t1)
     # ---- device only: the same K steps as bare C-ABI launches (b2g_task_step), same rotation: the kernel time
@@ -405,7 +428,7 @@ def run_gpu_arm(args):
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
     sink = torch.zeros(1, device=device)
     for k in range(args.steps):
-        flush.zero_()                      # write 256 MB (> 126 MB L2): evicts the previous step's tensors ...
+        flush.zero_()                      # write 256 MB (> 50 MB L2): evicts the previous step's tensors ...
         sink += flush.sum()                # ... then read it back: the dirty lines are written out, L2 is left clean and cold
         ev[k][0].record()
         env.sim.task_step(ring[k % 16])
@@ -467,16 +490,6 @@ def run_gpu_arm(args):
     peak, peak_kind = measured_peak()
     kernel_ms = dev_ms / args.steps
     achieved = n * bytes_per / (kernel_ms * 1e-3) / 1e9
-    traffic, flop = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            prof = json.load(f)
-        traffic = prof.get(args.workload)
-        flop = prof.get(args.workload + "_fp32_flop_per_launch")
-    except Exception:
-        pass
-    if flop is not None and n != WORKLOADS[args.workload][1]:
-        flop = flop * n / WORKLOADS[args.workload][1]
     quad = env.sim.quad_ns()
     line = {
         "metric": METRIC, "value": value, "unit": "env-steps/s", "n_gpus": world, "steps": args.steps,
@@ -484,7 +497,7 @@ def run_gpu_arm(args):
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"{task} num_envs={n} per GPU, random actions U(-1,1), sim dt {env.cfg['sim']['dt']} x {env.cfg['sim']['substeps']} substeps",
                    "num_envs_total": world * n, "env_sets": R,
-                   "timing": f"value = K x VecTask.step(actions) (device tensors) inside one CUDA-event pair on the launching stream; inputs larger than L2: {R} independent env sets of {n} envs stepped round-robin ({R * n * bytes_per / 1e6:.0f} MB of live tensors > 126 MB L2), so every step reads its state from HBM",
+                   "timing": f"value = K x VecTask.step(actions) (device tensors) inside one CUDA-event pair on the launching stream; inputs larger than L2: {R} independent env sets of {n} envs stepped round-robin ({R * n * bytes_per / 1e6:.0f} MB of live tensors > 50 MB L2), so every step reads its state from HBM",
                    "collective": "none on the step path; one NCCL all_gather of per-env returns per rollout (logging)",
                    "substep_formulation": f"quad (4 chains x {quad})" if quad else "generic slot program",
                    "parity": PARITY_NOTE},
@@ -500,7 +513,7 @@ def run_gpu_arm(args):
                 "h2d_bytes_per_step": n * A * 4, "d2h_bytes_per_step": n * (O * 4 + 4 + 8 + 1), "ms_per_step": e2e_ms / args.steps},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "peak_kind": peak_kind, "kernel_ms": kernel_ms,
+                     "peak_kind": peak_kind, "kernel_ms": kernel_ms,
                      "algorithmic_bytes_per_env_step": bytes_per},
         "clocks": clocks,
     }
@@ -510,10 +523,6 @@ def run_gpu_arm(args):
                            "note": "open-loop (random-action) rollout, the README benchmark's shape: all KR actions given up front, state stays on chip "
                                    "between the steps, every step's obs/reward/reset/time_out written to (KR, n, .) outputs; NOT the headline: a policy in "
                                    "the loop needs step()"}
-    if flop is not None:    # SURVEY 8d cross-check: the kernel is FP32-issue-bound, not HBM-bound
-        tf = flop / (kernel_ms * 1e-3) / 1e12
-        line["roofline"]["fp32"] = {"flop_per_launch": flop, "achieved": tf, "peak": 74.4, "unit": "TFLOP/s", "frac": tf / 74.4,
-                                    "note": "FFMA x2 + FADD + FMUL thread-instructions from the ncu capture in profiles/; peak = 148 SM x 128 lanes x 2 x 1.965 GHz"}
     if world == 1 and not args.no_cpu_baseline:
         cores = os.cpu_count() or 1
         est = {"Ant": 0.8e6, "Humanoid": 0.25e6, "Cartpole": 4e6, "AnymalTerrain": 0.15e6, "ShadowHand": 0.3e6}[task] * cores / 128.0
@@ -539,6 +548,8 @@ def main():
     ap.add_argument("--sets", type=int, default=0, help="independent env sets stepped round-robin (0 = enough to exceed 1.5 x L2)")
     ap.add_argument("--no-rollout", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write what the last timed step returned (obs, reward, reset, time_outs) as DIR/<name>.npy, float32")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":

@@ -1,9 +1,9 @@
 /*
- * b200gym.h -- C ABI of the B200-native vectorised environment stepper.
+ * b200gym.h -- C ABI of the CUDA-native (H100) vectorised environment stepper.
  *
  * The reference has no C FFI: its boundary for this path is the Python surface of the closed
  * `isaacgym` module (SURVEY.md 8b).  Each entry point below names the reference call it stands
- * behind (file:line under /root/reference/isaacgymenvs).  Conventions, taken from the call sites:
+ * behind (file:line under isaacgymenvs/ of the reference).  Conventions, taken from the call sites:
  *   - single caller thread, one sim per process is the common case (tasks/base/vec_task.py:58-64)
  *     but several handles may coexist;
  *   - all work is STREAM-ORDERED on the cudaStream_t passed in (the reference issues on the

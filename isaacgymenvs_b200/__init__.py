@@ -1,4 +1,4 @@
-"""B200-native vectorised environment stepper behind the IsaacGymEnvs surface.
+"""CUDA-native (H100) vectorised environment stepper behind the IsaacGymEnvs surface.
 
     import isaacgymenvs_b200 as isaacgymenvs
     envs = isaacgymenvs.make(seed=0, task="Ant", num_envs=16384, sim_device="cuda:0", rl_device="cuda:0")
@@ -32,7 +32,7 @@ def make(seed: int, task: str, num_envs: int, sim_device: str, rl_device: str, g
         task_cfg["rank"] = global_rank
     name = task_cfg.get("name", task)
     if name not in isaacgym_task_map:
-        raise KeyError(f"task {name!r} has no fused B200 kernel (supported: {sorted(isaacgym_task_map)})")
+        raise KeyError(f"task {name!r} has no fused CUDA kernel (supported: {sorted(isaacgym_task_map)})")
     return isaacgym_task_map[name](cfg=task_cfg, rl_device=rl_device, sim_device=sim_device,
                                    graphics_device_id=graphics_device_id, headless=headless,
                                    virtual_screen_capture=virtual_screen_capture, force_render=force_render)

@@ -1,6 +1,6 @@
 """Compiled articulation models.
 
-The robot descriptions (MJCF/URDF) live in the reference tree (`/root/reference/assets`), which
+The robot descriptions (MJCF/URDF) live in the reference tree (`assets/` of an IsaacGymEnvs checkout), which
 does not exist on the GPU box, so the importer's output is committed here as JSON
 (`compiled/*.json`, regenerate with `python -m isaacgymenvs_b200.assets.compile_assets`).  When a
 reference-style asset root is available `load_asset_file` parses the XML directly instead.

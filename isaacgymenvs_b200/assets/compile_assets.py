@@ -1,5 +1,5 @@
 """Regenerate compiled/*.json from the reference asset tree (run in the build container):
-    python -m isaacgymenvs_b200.assets.compile_assets [/root/reference/assets]
+    python -m isaacgymenvs_b200.assets.compile_assets <IsaacGymEnvs checkout>/assets
 AssetOptions per file are the ones the reference tasks pass:
 ant.py:149-152, humanoid.py:152-157, cartpole.py:84-88, anymal_terrain.py:218-231."""
 import os
@@ -28,7 +28,7 @@ SPECS = {
 }
 
 
-def main(root="/root/reference/assets"):
+def main(root):
     out = os.path.join(os.path.dirname(os.path.abspath(__file__)), "compiled")
     os.makedirs(out, exist_ok=True)
     for name, (rel, opts) in SPECS.items():

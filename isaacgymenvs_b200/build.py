@@ -1,4 +1,4 @@
-"""Builds libb200gym.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a."""
+"""Builds libb200gym.so (the C-ABI CUDA library) in-tree with nvcc for the H100 (sm_90a)."""
 import os
 import subprocess
 import sys
@@ -8,6 +8,13 @@ SRC = os.path.join(HERE, "csrc", "b200gym.cu")
 OUT = os.path.join(HERE, "libb200gym.so")
 DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("b2g_common.cuh", "b2g_device.cuh", "b2g_tasks.cuh", "b2g_anymal.cuh", "b2g_hand.cuh", "b2g_quad.cuh", "b2g_quad_kernels.cuh", "b2g_quad_host.h", "b2g_reset.cuh", "b2g_quad_rollout.cuh", "b2g_kin.cuh", "b2g_kin_host.h")
                 if os.path.exists(os.path.join(HERE, "csrc", f))] + [os.path.join(os.path.dirname(HERE), "include", "b200gym.h")]
+GENCODE = "arch=compute_90a,code=sm_90a"
+
+
+def _nvcc_cmd(out, defines=()):
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    return [nvcc, "-gencode", GENCODE, "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
+            "-Xcompiler", "-fPIC", "-shared", *defines, "-o", out, SRC]
 
 
 def needs_build():
@@ -20,9 +27,7 @@ def needs_build():
 def build(force=False, verbose=False, extra=()):
     if not force and not needs_build():
         return OUT
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-           "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared", "-o", OUT, SRC]
+    cmd = _nvcc_cmd(OUT)
     cmd += os.environ.get("B2G_NVCC_FLAGS", "").split()      # experiment hook
     if verbose:
         cmd += ["-Xptxas", "-v"]
@@ -37,9 +42,7 @@ def build_exact_trig(force=False):
     out = os.path.join(HERE, "libb200gym_exacttrig.so")
     if not force and os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in DEPS):
         return out
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
-                           "-Xcompiler", "-fPIC", "-shared", "-DB2G_FAST_TRIG=0", "-o", out, SRC])
+    subprocess.check_call(_nvcc_cmd(out, ["-DB2G_FAST_TRIG=0"]))
     return out
 
 

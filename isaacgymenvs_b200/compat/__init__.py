@@ -1,5 +1,5 @@
 """Compatibility path: run UNMODIFIED reference task files (which `import isaacgym` and subclass
-`isaacgymenvs.tasks.base.vec_task.VecTask`) on the B200 engine through the generic `gym.*` tensor
+`isaacgymenvs.tasks.base.vec_task.VecTask`) on the CUDA engine through the generic `gym.*` tensor
 API -- Python hooks run as they are, `gym.simulate` is the CUDA physics kernel (SURVEY.md 8f rank 2).
 
     from isaacgymenvs_b200 import compat

@@ -1,4 +1,4 @@
-"""`isaacgym.gymapi` look-alike backed by the B200 engine (SURVEY.md 8b "required exports").
+"""`isaacgym.gymapi` look-alike backed by the CUDA engine (SURVEY.md 8b "required exports").
 
 Only what `tasks/base/vec_task.py`, the single-actor-per-env tasks and ShadowHand's three-actor envs (articulation +
 free box + gravity-less marker, `shadow_hand.py:338-383`) touch is provided; every method cites a representative call site.  Actors, assets and envs are RECORDED

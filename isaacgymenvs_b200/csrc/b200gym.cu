@@ -1,5 +1,5 @@
-// b200gym.cu -- kernels + C ABI (include/b200gym.h) of the B200-native environment stepper.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -shared -Xcompiler -fPIC
+// b200gym.cu -- kernels + C ABI (include/b200gym.h) of the CUDA-native (H100) environment stepper.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -shared -Xcompiler -fPIC
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1148,11 +1148,13 @@ extern "C" int b2g_refresh_kinematic_tensors(b2g_sim *s, int32_t which, void *st
     float *M = (which & B2G_KIN_MASS_MATRIX) ? (float *)s->buf.p[B2G_T_MASS_MATRIX] : nullptr;
     // one warp per env -- or per two envs when links and bodies fit 16 lanes (arms, quadrupeds); at most a few resident waves of
     // CTAs, the warps stride over the envs
+    int sms = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device));
     if (s->hk.nl <= 16 && s->hk.nb <= 16) {
-        const int grid = std::min((N + 2 * WARPS - 1) / (2 * WARPS), 148 * 8);
+        const int grid = std::min((N + 2 * WARPS - 1) / (2 * WARPS), sms * 8);
         kin_tensors_kernel<WARPS, 16><<<grid, WARPS * 32, 0, (cudaStream_t)stream>>>(s->d_kin, root, dof, J, M, N);
     } else {
-        const int grid = std::min((N + WARPS - 1) / WARPS, 148 * 8);
+        const int grid = std::min((N + WARPS - 1) / WARPS, sms * 8);
         kin_tensors_kernel<WARPS, 32><<<grid, WARPS * 32, 0, (cudaStream_t)stream>>>(s->d_kin, root, dof, J, M, N);
     }
     s->launches++;

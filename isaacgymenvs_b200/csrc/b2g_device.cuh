@@ -1,4 +1,4 @@
-// b2g_device.cuh -- device-side articulated-body sub-step (sm_100a).
+// b2g_device.cuh -- device-side articulated-body sub-step (sm_90a).
 //
 // Replaces the closed `gym.simulate(sim)` (call sites tasks/base/vec_task.py:379-382,
 // tasks/anymal_terrain.py:448 in the reference) with the algorithm BASELINE.json's north_star names:
@@ -21,8 +21,7 @@
 // 128-bit accesses) or, for the multi-actor kernels, [link][k][env] (no storage for idle slots) --
 // and the articulated inertia being swept travels in registers along chains, through parked
 // accumulators otherwise.  This keeps the kernel ~1/5 the code size and ~1/2 the registers of the
-// fully unrolled first version (profiles/r1_v1_*: 88 KB of SASS, 255 registers, 24 % of issue stalls
-// "no instruction").
+// fully unrolled first version.
 //
 // OBJ = true adds a second, free rigid body per env (a box: ShadowHand's cube) in contact with the
 // articulation's spheres and box primitives and with the ground, plus fixed two-joint tendons.

@@ -1,4 +1,4 @@
-// b2g_kin.cuh -- Jacobian and joint-space mass-matrix tensors (sm_100a).
+// b2g_kin.cuh -- Jacobian and joint-space mass-matrix tensors (sm_90a).
 //
 // Stands behind gym.acquire_jacobian_tensor / acquire_mass_matrix_tensor + refresh_jacobian_tensors /
 // refresh_mass_matrix_tensors (reference call sites tasks/franka_cube_stack.py:388-392,439-440; consumer: the
@@ -40,9 +40,8 @@ struct alignas(16) KinModel {
     float mass[MAX_LINKS], armature[MAX_LINKS], body_pos[MAX_LINKS][3];
 };
 
-// per-warp scratch.  Everything a phase hands to another lane is packed into float4 rows: the profile of the first version
-// (profiles/r2_kin_humanoid_ncu_summary.json) showed the LSU pipe 77 % busy with 32-bit shared loads -- one 128-bit load moves
-// four of them.  Lane-indexed accesses at a stride of 3 float4 (12 words) are conflict-free per quarter-warp.
+// per-warp scratch.  Everything a phase hands to another lane is packed into float4 rows: the first version
+// kept the LSU pipe busy with 32-bit shared loads -- one 128-bit load moves four of them.  Lane-indexed accesses at a stride of 3 float4 (12 words) are conflict-free per quarter-warp.
 struct KinScratch {
     float4 Rx[MAX_LINKS][3];        // row k: (R[k][0], R[k][1], R[k][2], x[k]) -- link frame in world axes, origin relative to the root origin O
     float4 S[MAX_LINKS][3];         // (n.xyz, f.x) (f.yz, sa.xy) (sa.z, sb.xyz): Ic_i S_i = (n ; f) and the motion subspace S = (sa ; sb) about O

@@ -3,9 +3,8 @@
 // reference call sites tasks/base/vec_task.py:379-382, tasks/anymal_terrain.py:448) as STRAIGHT-LINE code.
 //
 // Why a second formulation of the same sub-step: the generic Stepper interprets a slot program (rolled loops,
-// per-slot records, 10 float4 of shared-memory state per link and pass, runtime joint-type flags).  ncu on the
-// round-1 Ant kernel (profiles/r1_ant_v4_*): 13.55 M warp-instructions per launch, 6 600 per warp, of which the
-// floating-point work is about half -- the rest is addressing, loop control, flag tests and shared-memory
+// per-slot records, 10 float4 of shared-memory state per link and pass, runtime joint-type flags).  In its Ant
+// kernel the floating-point work is about half of the instructions -- the rest is addressing, loop control, flag tests and shared-memory
 // traffic.  Here the chain length NS is a template parameter, everything a lane needs between the sweeps stays
 // in registers, the model constants arrive as conflict-free 128-bit shared-memory loads ([k][leg] layout), the
 // joint rotation is three constant matrices (Rj = M0 + cos q M1 + sin q M2, so no per-joint Rodrigues on matrix

@@ -1,6 +1,6 @@
 // b2g_tasks.cuh -- per-task observation / reward / reset arithmetic, fused behind the physics.
 //
-// Each function restates (file:line under /root/reference/isaacgymenvs) the @torch.jit.script
+// Each function restates (file:line under isaacgymenvs/ of the reference) the @torch.jit.script
 // function it replaces and keeps its OPERATION ORDER: tests compare against golden vectors produced
 // by the reference's own functions (tests/golden) at 1e-6, and `potentials` bit-exactly, because
 // progress_reward = potentials - prev_potentials (tasks/ant.py:359) differences two ~6e4 numbers.

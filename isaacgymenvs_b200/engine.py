@@ -260,7 +260,7 @@ class Sim:
         self.num_envs = int(num_envs)
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise EngineError("the B200 engine has no CPU path: device must be a CUDA device")
+            raise EngineError("the CUDA engine has no CPU path: device must be a CUDA device")
         self.nd, self.nb, self.ns = model.ndof, model.nb, len(model.sensor_body)
         cm, self._keep = pack_model(model, ground_mu)
         sp = CSimParams()

@@ -226,7 +226,7 @@ class Model:
         return d
 
     # ---- (de)serialisation: committed under assets/compiled/*.json so the GPU box, which has no
-    # /root/reference, can build the same model
+    # the reference checkout, can build the same model
     def to_json(self):
         out = {}
         for k, v in self.__dict__.items():

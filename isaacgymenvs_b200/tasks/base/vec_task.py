@@ -150,7 +150,7 @@ class VecTask(Env):
             self.randomizer = Randomizer(task_cfg.get("randomization_params", {}))
         if self.device == "cpu":
             raise engine.EngineError(
-                "sim_device=cpu / pipeline=cpu: the B200-native stepper has no CPU path (north_star: no CPU "
+                "sim_device=cpu / pipeline=cpu: the CUDA-native stepper has no CPU path (north_star: no CPU "
                 "fallback); the CPU restatement lives in oracle/ and is only driven by tests and bench.py")
         self.seed = int(self.cfg.get("seed", 42)) if isinstance(self.cfg, dict) else 42
         self.env_id_offset = int(self.cfg.get("env_id_offset", 0))

@@ -10,7 +10,7 @@ from ..assets import load_asset_file
 from ..importer.model import BuildOptions, enable_self_collision
 from .base.vec_task import VecTask
 
-_ASSET_ROOT_CANDIDATES = [os.environ.get("B2G_ASSET_ROOT", ""), "/root/reference/assets"]
+_ASSET_ROOT_CANDIDATES = [os.environ.get("B2G_ASSET_ROOT", "")]
 
 
 def _asset_root():

@@ -1,7 +1,7 @@
 """Height-field terrain generator for AnymalTerrain.
 
 The reference builds its terrain with `isaacgym.terrain_utils` (`tasks/anymal_terrain.py:542-653`),
-which ships inside the closed Isaac Gym package and is not under /root/reference.  The generators
+which ships inside the closed Isaac Gym package and is not under the reference checkout.  The generators
 below are restated from what the call sites require (argument meaning, units, the SubTerrain
 fields they touch) and the published behaviour of those helpers: integer height samples
 (`vertical_scale` metres per unit) on a `horizontal_scale` grid.  Exact sample-for-sample equality

@@ -5,9 +5,9 @@
  * load this library; the product path (isaacgymenvs_b200/csrc) never does.
  *
  * PARITY UNPINNED against the reference: the function this restates, `gym.simulate(sim)`
- * (call sites /root/reference/isaacgymenvs/tasks/base/vec_task.py:379-382 and
+ * (call sites isaacgymenvs/ of the reference/tasks/base/vec_task.py:379-382 and
  * tasks/anymal_terrain.py:448), lives in the closed Isaac Gym Preview 4 / PhysX binary, which is
- * absent from /root/reference and cannot be installed here (SURVEY.md 8c).  The reference holds no
+ * absent from the reference checkout and cannot be installed here (SURVEY.md 8c).  The reference holds no
  * golden vectors for it.  What this file pins instead is the algorithm BASELINE.json's north_star
  * prescribes -- Featherstone ABA, PD/effort actuators, semi-implicit Euler, penalty contact -- and
  * it is itself pinned by (tests/test_oracle_physics.py) an independent numpy RNEA inverse-dynamics

@@ -1,8 +1,8 @@
 """Generate golden input/output vectors from the REFERENCE's own @torch.jit.script functions.
 
-Run in the build container only (needs /root/reference):
+Run in the build container only (needs an IsaacGymEnvs checkout named by ISAACGYMENVS_ROOT):
     python tests/golden/make_golden.py
-The reference task modules are loaded BY PATH from /root/reference with `isaacgym` and the VecTask
+The reference task modules are loaded BY PATH from that checkout with `isaacgym` and the VecTask
 base stubbed out (SURVEY.md 8c) -- nothing is copied.  Outputs: tests/golden/*.npz (committed).
 Pins: compute_ant_observations / compute_ant_reward (tasks/ant.py:325-408),
 compute_humanoid_observations / compute_humanoid_reward (tasks/humanoid.py:323-413),
@@ -16,7 +16,7 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/isaacgymenvs"
+REF = os.path.join(os.environ.get("ISAACGYMENVS_ROOT", "."), "isaacgymenvs")     # an IsaacGymEnvs checkout
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

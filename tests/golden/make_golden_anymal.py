@@ -12,7 +12,7 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/isaacgymenvs"
+REF = os.path.join(os.environ.get("ISAACGYMENVS_ROOT", "."), "isaacgymenvs")     # an IsaacGymEnvs checkout
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

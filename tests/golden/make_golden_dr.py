@@ -13,7 +13,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("ISAACGYMENVS_ROOT", ".")     # an IsaacGymEnvs checkout
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 CASES = {

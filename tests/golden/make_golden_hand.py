@@ -16,7 +16,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/isaacgymenvs"
+REF = os.path.join(os.environ.get("ISAACGYMENVS_ROOT", "."), "isaacgymenvs")     # an IsaacGymEnvs checkout
 OUT = os.path.dirname(os.path.abspath(__file__))
 SEED = 42
 

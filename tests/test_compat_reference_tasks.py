@@ -1,5 +1,5 @@
-"""The compatibility path on CPU: the reference's UNMODIFIED task files (loaded from
-/root/reference, never copied) import against the `isaacgym` shim and run their own Python hooks --
+"""The compatibility path on CPU: the reference's UNMODIFIED task files (staged by build()
+from an IsaacGymEnvs checkout into oracle/_ref/, or read from the checkout ISAACGYMENVS_ROOT names; never committed) import against the `isaacgym` shim and run their own Python hooks --
 create_sim / pre_physics_step / post_physics_step / reset_idx / jit obs+reward -- through the
 hook-style VecTask.  The engine itself needs a GPU, so here `engine.Sim` is replaced by a stand-in
 with the same tensors whose `simulate()` integrates nothing: what is tested is the API surface, the
@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.conftest import needs_reference, REFERENCE
+from tests.conftest import needs_checkout, CHECKOUT, REFERENCE
 
 
 class _FakeSim:
@@ -52,7 +52,7 @@ def compat_cpu(monkeypatch):
         if k.startswith("isaacgymenvs.") or k in ("isaacgym", "isaacgymenvs") or k.startswith("isaacgym."):
             if not k.startswith("isaacgymenvs_b200"):
                 del sys.modules[k]
-    compat.install(reference_root=REFERENCE)
+    compat.install(reference_root=CHECKOUT)
     monkeypatch.setattr(engine, "Sim", _FakeSim)
     vec_task_hooks.reset_sim_singleton()
     yield
@@ -72,13 +72,13 @@ def _cfg(task, n):
     return t
 
 
-@needs_reference
+@needs_checkout
 @pytest.mark.parametrize("task,module,cls,nobs,nact", [("Ant", "ant", "Ant", 60, 8), ("Humanoid", "humanoid", "Humanoid", 108, 21),
                                                        ("Cartpole", "cartpole", "Cartpole", 4, 1)])
 def test_unmodified_reference_task_runs_on_the_shim(compat_cpu, task, module, cls, nobs, nact):
     import importlib
     mod = importlib.import_module(f"isaacgymenvs.tasks.{module}")          # the reference's own file
-    assert os.path.realpath(mod.__file__).startswith(REFERENCE)
+    assert os.path.realpath(mod.__file__).startswith(os.path.realpath(CHECKOUT))
     n = 16
     env = getattr(mod, cls)(cfg=_cfg(task, n), rl_device="cpu", sim_device="cpu", graphics_device_id=-1, headless=True,
                             virtual_screen_capture=False, force_render=False)
@@ -103,13 +103,13 @@ def test_unmodified_reference_task_runs_on_the_shim(compat_cpu, task, module, cl
     assert (env.progress_buf == 1).all()
 
 
-@needs_reference
+@needs_checkout
 def test_unmodified_reference_shadow_hand_runs_on_the_shim(compat_cpu):
     """Three actors per env (hand, cube, goal marker), tendon properties, actor-indexed setters, the 211-d full_state
     observation: the reference's own shadow_hand.py drives the shim unmodified."""
     import importlib
     mod = importlib.import_module("isaacgymenvs.tasks.shadow_hand")
-    assert os.path.realpath(mod.__file__).startswith(REFERENCE)
+    assert os.path.realpath(mod.__file__).startswith(os.path.realpath(CHECKOUT))
     n = 8
     env = mod.ShadowHand(cfg=_cfg("ShadowHand", n), rl_device="cpu", sim_device="cpu", graphics_device_id=-1, headless=True,
                          virtual_screen_capture=False, force_render=False)
@@ -137,7 +137,6 @@ def test_unmodified_reference_shadow_hand_runs_on_the_shim(compat_cpu):
     assert "consecutive_successes" in extras and "time_outs" in extras
 
 
-@needs_reference
 def test_procedural_primitive_assets_become_the_free_object(compat_cpu):
     """gym.create_sphere / create_box / create_capsule (ball_balance.py:277, franka_cube_stack.py:223-245): one primitive, mass =
     density x volume, and as the second actor of an env the engine's rounded box (sphere: a point + radius)."""
@@ -170,7 +169,7 @@ def test_procedural_primitive_assets_become_the_free_object(compat_cpu):
     assert torch.allclose(rs[:, 1, 0:3], torch.tensor([0.5, 0.0, 1.0]))
 
 
-@needs_reference
+@needs_checkout
 def test_name_maps_and_small_accessors_of_the_shim(compat_cpu):
     """the dictionary / count accessors other reference tasks use around the tensor API (franka_cube_stack.py:391, allegro_hand.py,
     ant.py:307-321 debug lines): body / DOF order = the tensors' order"""
@@ -193,7 +192,7 @@ def test_name_maps_and_small_accessors_of_the_shim(compat_cpu):
     gym.add_lines(None, None, 0, [], []); gym.clear_lines(None); gym.debug_print_asset(sim.asset)
 
 
-@needs_reference
+@needs_checkout
 def test_reference_shadow_hand_random_forces_reach_the_engine(compat_cpu):
     """env.forceScale > 0 (shadow_hand.py:700-709): the reference's own pre_physics_step calls
     apply_rigid_body_force_tensors(rb_forces, None, LOCAL_SPACE); the shim hands the object's row to the engine for
@@ -229,7 +228,7 @@ def test_reference_shadow_hand_random_forces_reach_the_engine(compat_cpu):
     assert torch.allclose(sim.tensors[sim.E.T_OBJ_FORCE], quat_rotate_inverse(q, f[:, obj]), atol=1e-6)
 
 
-@needs_reference
+@needs_checkout
 @pytest.mark.parametrize("obj,half,rnd,mass", [("pen", [0.0, 0.0, 0.1], 0.008, 0.042357), ("egg", [0.0, 0.0, 0.01], 0.03, 0.150796)])
 def test_reference_shadow_hand_egg_and_pen_reach_the_engine_as_rounded_boxes(compat_cpu, obj, half, rnd, mass):
     """env.objectType egg / pen (shadow_hand.py:84-99): the reference loads egg.xml / pen.xml itself; the shim turns the single
@@ -249,13 +248,13 @@ def test_reference_shadow_hand_egg_and_pen_reach_the_engine_as_rounded_boxes(com
     assert torch.isfinite(obs["obs"]).all()
 
 
-@needs_reference
+@needs_checkout
 def test_unmodified_reference_flat_anymal_runs_on_the_shim(compat_cpu):
     """SURVEY 8f rank 2: tasks/anymal.py drives PhysX position drives (DOF_MODE_POS via set_actor_dof_properties,
     set_dof_position_target_tensor) and reads net contact forces -- unmodified on the shim."""
     import importlib
     mod = importlib.import_module("isaacgymenvs.tasks.anymal")
-    assert os.path.realpath(mod.__file__).startswith(REFERENCE)
+    assert os.path.realpath(mod.__file__).startswith(os.path.realpath(CHECKOUT))
     n = 8
     env = mod.Anymal(cfg=_cfg("Anymal", n), rl_device="cpu", sim_device="cpu", graphics_device_id=-1, headless=True,
                      virtual_screen_capture=False, force_render=False)
@@ -269,13 +268,13 @@ def test_unmodified_reference_flat_anymal_runs_on_the_shim(compat_cpu):
     assert torch.allclose(sim.dof_target, 0.5 * env.actions + env.default_dof_pos)
 
 
-@needs_reference
+@needs_checkout
 def test_unmodified_reference_anymal_terrain_runs_on_the_shim(compat_cpu):
     """tasks/anymal_terrain.py builds its terrain with isaacgym.terrain_utils (restated in isaacgymenvs_b200/terrain.py),
     converts it to a triangle mesh and calls gym.add_triangle_mesh; the shim hands the engine the underlying height field."""
     import importlib
     mod = importlib.import_module("isaacgymenvs.tasks.anymal_terrain")
-    assert os.path.realpath(mod.__file__).startswith(REFERENCE)
+    assert os.path.realpath(mod.__file__).startswith(os.path.realpath(CHECKOUT))
     n = 16
     cfg = _cfg("AnymalTerrain", n)
     cfg["env"]["terrain"]["numLevels"] = 2; cfg["env"]["terrain"]["numTerrains"] = 2

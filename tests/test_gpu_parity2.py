@@ -287,17 +287,13 @@ def test_hand_baseline_size_simulate_matches_oracle():
 
 
 # ------------------------------------------------------------------------------------ fast trigonometry
-def test_fast_trig_build_is_bounded_against_exact_trig_build():
+def test_fast_trig_build_is_bounded_against_exact_trig_build(tmp_path):
     """The product build evaluates joint rotations with __sincosf (B2G_FAST_TRIG=1).  Same library built with sincosf:
     one control step from states that include joint angles AT and beyond the limits (|q| up to 2.8 rad for the
     Humanoid knee) differs by < 2e-5 in base pose, < 1e-4 in joint positions (90 % below 1e-5, median below 1e-6) and < 5e-3 relative in joint velocities; after 30-step
     rollouts the median env is still within 1e-3 of its twin."""
-    exact = os.path.join(ROOT, "isaacgymenvs_b200", "libb200gym_exacttrig.so")
     from isaacgymenvs_b200 import build as B
-    if not os.path.exists(exact) or any(os.path.getmtime(d) > os.path.getmtime(exact) for d in B.DEPS):   # same ABI as the product build
-        cmd = [os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared", "-DB2G_FAST_TRIG=0", "-o", exact, B.SRC]
-        subprocess.check_call(cmd)
+    exact = B.build_exact_trig()                                    # same ABI as the product build; rebuilt only when stale
     code = r'''
 import os, sys, copy, numpy as np, torch
 sys.path.insert(0, %r)
@@ -331,7 +327,7 @@ np.savez(sys.argv[1], **out)
 ''' % ROOT
     res = []
     for lib in ("", exact):
-        out = os.path.join("/tmp", f"b2g_trig_{int(bool(lib))}.npz")
+        out = str(tmp_path / f"b2g_trig_{int(bool(lib))}.npz")
         env_ = dict(os.environ)
         if lib:
             env_["B2G_LIB"] = lib
@@ -343,7 +339,7 @@ np.savez(sys.argv[1], **out)
         d1f = fast[name + "_dof1"].reshape(512, -1, 2); d1e = ex[name + "_dof1"].reshape(512, -1, 2)
         dq1 = np.abs(d1f[..., 0] - d1e[..., 0])
         dv1 = np.abs(d1f[..., 1] - d1e[..., 1]) / np.maximum(1, np.abs(d1e[..., 1]))
-        # measured on B200 (Ant): worst DOF 3.7e-5 rad / 2.0e-3 relative in velocity -- a foot pressed into the ground, where the
+        # Ant: worst DOF 3.7e-5 rad / 2.0e-3 relative in velocity -- a foot pressed into the ground, where the
         # contact spring amplifies the 5e-7 absolute error of __sincosf; the 4 worst of 4096 DOFs reach 2.7e-5 rad; the bulk is
         # at rounding level
         assert dq1.max() < 1e-4 and np.quantile(dq1, 0.9) < 1e-5 and np.median(dq1) < 1e-6, (dq1.max(), np.quantile(dq1, 0.9), np.median(dq1))

@@ -1,5 +1,5 @@
 """CPU-side checks that need no GPU: the C-ABI library builds, loads and exports every symbol
-include/b200gym.h declares; the config loaders agree with the reference's YAML; importer
+include/b200gym.h declares; the config loaders agree with the reference's YAML (tests/golden/reference_data.tar.xz); importer
 known-answers; the engine refuses to run without a CUDA device (no CPU fallback)."""
 import ctypes
 import os
@@ -7,7 +7,7 @@ import re
 import numpy as np
 import pytest
 
-from tests.conftest import needs_reference, REFERENCE, ROOT
+from tests.conftest import REFERENCE, ROOT
 
 
 def test_library_builds_and_exports_the_declared_abi():
@@ -47,7 +47,6 @@ def test_no_cpu_fallback():
         engine.Sim(load_compiled("ant"), 4, 0.0166, 2, device="cpu")
 
 
-@needs_reference
 @pytest.mark.parametrize("task", ["Cartpole", "Ant", "Humanoid", "ShadowHand"])
 def test_reference_yaml_loads_unmodified_and_matches_builtin(task):
     from isaacgymenvs_b200 import config
@@ -66,7 +65,6 @@ def test_reference_yaml_loads_unmodified_and_matches_builtin(task):
     assert ref["task"]["sim"]["physx"]["num_threads"] == 4
 
 
-@needs_reference
 def test_importer_known_answers_and_compiled_blobs_are_current():
     """SURVEY.md 8c importer known-answers (analytic, from the XML) + committed blobs == fresh import."""
     from isaacgymenvs_b200.importer.mjcf import load_mjcf
@@ -301,7 +299,6 @@ def test_train_launcher_maps_reference_overrides():
             tr.to_ppo_argv(tr.parse_overrides(bad))
 
 
-@needs_reference
 def test_train_launcher_hyperparameters_are_the_reference_yaml():
     import importlib.util, yaml
     spec = importlib.util.spec_from_file_location("b2g_train", os.path.join(ROOT, "train.py"))
@@ -344,7 +341,6 @@ def test_mesh_mass_properties_are_those_of_the_enclosed_solid(tmp_path):
         mass_properties(np.zeros((3, 3)), np.array([[0, 1, 2]]))
 
 
-@needs_reference
 def test_franka_links_get_their_mass_from_the_collision_meshes():
     """franka_panda_gripper.urdf has no <inertial>: density x mesh volume (AssetOptions.density 1000) must give a ~20 kg arm, and
     the skipped mesh CONTACT is announced, not silent."""

@@ -285,10 +285,9 @@ def test_mass_matrix_is_the_inertia_the_aba_step_inverts(name):
 
 # ---------------------------------------------------------------------------------------------------------------
 # the reference's indexing idiom for the operational-space controller (franka_cube_stack.py:388-394, 600-627) on the Franka itself
-from tests.conftest import needs_reference, REFERENCE
+from tests.conftest import REFERENCE
 
 
-@needs_reference
 def test_franka_jacobian_is_indexed_by_joint_as_the_reference_does():
     """`hand_joint_index = gym.get_actor_joint_dict(env, franka)['panda_hand_joint']; j_eef = jacobian[:, hand_joint_index, :, :7]`:
     with one joint per non-root body the joint index addresses the hand body's row of the fixed-base Jacobian.  Checked on the

@@ -1,7 +1,7 @@
 """CPU test of the quad sub-step (isaacgymenvs_b200/csrc/b2g_quad.cuh): the header is __host__ __device__, so
 tests/quad_host.cu compiles it for the HOST and runs the arithmetic the CUDA kernels execute, lane by lane, against the
 fp64 oracle -- same states, same tolerances as tests/test_gpu_parity.py::test_simulate_matches_oracle.  No GPU needed:
-a wrong term in the specialised Ant / ANYmal step shows up here, before any B200 time is spent."""
+a wrong term in the specialised Ant / ANYmal step shows up here, before any GPU time is spent."""
 import copy
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-"""Condense one kernel of an ncu capture into the JSON summaries kept under profiles/.
+"""Condense one kernel of an ncu capture into a JSON summary.
     python tools/ncu_summary.py <report.ncu-rep> <kernel-name substring> <out.json> ["free-text note"]
 Reads `ncu -i <rep> --page raw --csv`; the first launch whose name contains the substring is summarised."""
 import csv, io, json, subprocess, sys

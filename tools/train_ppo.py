@@ -7,7 +7,7 @@ minibatch 32768, 4 mini-epochs, e_clip 0.2, critic_coef 2, normalised inputs / v
 bounds loss 1e-4).  rl_games itself is not installable here (no network); this is the smallest learner that exercises
 the same contract and answers the question the parity tests cannot: does Ant LEARN on this physics?
 
-    python tools/train_ppo.py --task Ant --num-envs 4096 --epochs 500 --out profiles/r2_ppo_ant.json
+    python tools/train_ppo.py --task Ant --num-envs 4096 --epochs 500 --out ppo_ant.json
 """
 import argparse
 import json
