@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "b200gym.cu")
 OUT = os.path.join(HERE, "libb200gym.so")
-DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("b2g_common.cuh", "b2g_device.cuh", "b2g_tasks.cuh", "b2g_anymal.cuh", "b2g_hand.cuh", "b2g_quad.cuh", "b2g_quad_kernels.cuh", "b2g_quad_host.h", "b2g_reset.cuh", "b2g_quad_rollout.cuh", "b2g_kin.cuh", "b2g_kin_host.h")
+DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("b2g_common.cuh", "b2g_device.cuh", "b2g_tasks.cuh", "b2g_anymal.cuh", "b2g_hand.cuh", "b2g_quad.cuh", "b2g_quad_kernels.cuh", "b2g_quad_host.h", "b2g_model_host.h", "b2g_reset.cuh", "b2g_quad_rollout.cuh", "b2g_kin.cuh", "b2g_kin_host.h")
                 if os.path.exists(os.path.join(HERE, "csrc", f))] + [os.path.join(os.path.dirname(HERE), "include", "b200gym.h")]
 GENCODE = "arch=compute_90a,code=sm_90a"
 

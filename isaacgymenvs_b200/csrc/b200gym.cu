@@ -7,6 +7,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <memory>
 
 #include "../../include/b200gym.h"
 #include "b2g_device.cuh"
@@ -523,7 +524,7 @@ __global__ void __launch_bounds__(BLOCK) cartpole_step_kernel(const DevModel *__
 #include "b2g_anymal.cuh"
 #include "b2g_hand.cuh"
 #include "b2g_quad_kernels.cuh"
-#include "b2g_quad_host.h"
+#include "b2g_model_host.h"
 #include "b2g_reset.cuh"
 #include "b2g_quad_rollout.cuh"
 
@@ -590,17 +591,15 @@ __global__ void __launch_bounds__(128) body_state_kernel(const DevModel *__restr
 // ============================================================================================
 // host side
 // ============================================================================================
-struct b2g_sim {
+struct b2g_sim : SimModel {
     int device = 0;
     int num_envs = 0;
-    int lanes = 1;
-    int block = 128;             // threads per CTA, chosen so the slot state fits in shared memory
-    size_t dyn_smem = 0;
-    DevModel hm;                 // host copy
-    DevModel *dm = nullptr;      // device copy
+    DevModel *dm = nullptr;      // device copy of hm
     int16_t *d_hf = nullptr;
-    Buffers buf;
-    size_t buf_bytes[B2G_T_COUNT];
+    float4 *d_qm = nullptr;      // device copy of qm
+    KinModel *d_kin = nullptr;   // device copy of hk
+    Buffers buf = {};
+    size_t buf_bytes[B2G_T_COUNT] = {};
     b2g_task_params task;
     b2g_anymal_params anymal;
     b2g_hand_params hand;
@@ -608,19 +607,16 @@ struct b2g_sim {
     bool has_task = false, has_anymal = false, has_hand = false;
     unsigned step_counter = 0;   // common_step_counter, anymal_terrain.py:459
     float *d_actions_stage = nullptr;    // device staging for b2g_task_step_host
-    struct { bool on = false; float *obs = nullptr, *rew = nullptr; long long *reset = nullptr; uint8_t *timeout = nullptr; } zero_copy;
     int64_t launches = 0;
-    // quad path (b2g_quad.cuh): chain length (2 Ant-like, 3 ANYmal-like) or 0 = generic Stepper; the packed constants
-    int quad_ns = 0;
-    int quad_spec = 0;                        // QLane specialisation flags the constants are packed for (b2g_quad.cuh)
-    int quad_block = 64;                      // threads per CTA of the quad step kernels (B2G_QUAD_BLOCK: 32 / 64 / 128)
-    float4 *d_qm = nullptr;
-    KinModel hk;                              // constant tables of the Jacobian / mass-matrix kernel (b2g_kin.cuh)
-    KinModel *d_kin = nullptr;
-    bool kin_ok = false;
     std::vector<const void *> smem_set;      // kernels whose dynamic shared-memory limit has been raised (once per sim)
-    bool no_zero_copy = false;
-    size_t hostio_pad = 0;                    // extra dynamic shared memory of the host-I/O Ant launch (see b2g_task_step_host)
+
+    b2g_sim() = default;
+    b2g_sim(const b2g_sim &) = delete;
+    b2g_sim &operator=(const b2g_sim &) = delete;
+    ~b2g_sim() {
+        cudaSetDevice(device);
+        for (void *p : {(void *)dm, (void *)d_hf, (void *)d_qm, (void *)d_kin, (void *)d_actions_stage}) if (p) cudaFree(p);
+    }
 };
 
 static thread_local std::string g_err;
@@ -631,91 +627,6 @@ extern "C" const char *b2g_last_error(void) { return g_err.c_str(); }
 extern "C" int b2g_version(void) { return B2G_VERSION; }
 extern "C" int64_t b2g_launch_count(const b2g_sim *sim) { return sim ? sim->launches : 0; }
 extern "C" int b2g_quad_chain_length(const b2g_sim *sim) { return sim ? sim->quad_ns : 0; }
-
-// Build the lanes' slot programs: list-schedule the links over `L` lanes, critical path first; a lane
-// keeps following a chain (parent at step s-1 in the same lane -> state travels in registers), any
-// other parent/child relation goes through shared memory (parked inertia / pose / acceleration).
-static int schedule(const b2g_model *m, int L, DevModel &h, bool compact = false) {
-    const int nl = m->nl;
-    std::vector<int> height(nl, 1);
-    for (int i = nl - 1; i >= 1; i--) height[m->parent[i]] = std::max(height[m->parent[i]], height[i] + 1);
-    std::vector<int> t_of(nl, -1), lane_of(nl, -1);
-    t_of[0] = -1;
-    std::vector<int> lane_last(L, -1);
-    int remaining = nl - 1, t = 0;
-    for (int s = 0; s < MAX_SLOTS; s++) for (int l = 0; l < MAX_LANES; l++) {
-        SlotRec &r = h.slots[s][l]; r.link = -1; r.parent = 0; r.out = -1; r.flags = 0;
-        for (int c = 0; c < MAX_CHILD_REFS; c++) r.child[c] = -1;
-    }
-    while (remaining > 0) {
-        if (t >= MAX_SLOTS) return -1;
-        std::vector<int> ready;
-        for (int i = 1; i < nl; i++) if (t_of[i] < 0 && (m->parent[i] == 0 || (t_of[m->parent[i]] >= 0 && t_of[m->parent[i]] < t))) ready.push_back(i);
-        std::stable_sort(ready.begin(), ready.end(), [&](int a, int b) { return height[a] > height[b]; });
-        std::vector<int> pick(L, -1);
-        std::vector<char> used(nl, 0);
-        for (int l = 0; l < L; l++) {                                   // continue chains first
-            if (lane_last[l] < 0) continue;
-            for (int i : ready) if (!used[i] && m->parent[i] == lane_last[l]) { pick[l] = i; used[i] = 1; break; }
-        }
-        for (int i : ready) {                                            // then the most critical remaining links
-            if (used[i]) continue;
-            int l = 0; while (l < L && pick[l] >= 0) l++;
-            if (l == L) break;
-            pick[l] = i; used[i] = 1;
-        }
-        for (int l = 0; l < L; l++) {
-            lane_last[l] = pick[l];
-            if (pick[l] >= 0) { t_of[pick[l]] = t; lane_of[pick[l]] = l; h.slots[t][l].link = pick[l]; remaining--; }
-        }
-        t++;
-    }
-    h.ns = t; h.lanes = L; h.cross_lane = 0; h.root_acc = -1;
-    std::vector<int> nacc(L, 0);
-    bool need_root_acc = false;
-    for (int i = 1; i < nl; i++) if (m->parent[i] == 0 && t_of[i] > 0) need_root_acc = true;
-    // compact (env-wide) accumulator ids: per-lane ones take L consecutive ids, parked inertias one each
-    int gacc = 0;
-    if (compact && m->root_fixed) need_root_acc = false;                 // nothing collects a fixed root's children
-    if (need_root_acc) { h.root_acc = 0; for (int l = 0; l < L; l++) nacc[l] = 1; gacc = L; }
-    for (int i = 1; i < nl; i++) {
-        const int l = lane_of[i], s = t_of[i], p = m->parent[i];
-        SlotRec &r = h.slots[s][l];
-        if (p == 0) {
-            r.parent = 0;
-            r.out = (s == 0) ? -1 : h.root_acc;
-            if (compact && m->root_fixed) r.out = (s == 0) ? -1 : -2;
-        } else {
-            const int lp = lane_of[p], sp = t_of[p];
-            r.parent = (lp << 8) | (sp + 1);
-            if (lp != l) h.cross_lane = 1;
-            if (lp == l && sp == s - 1) r.out = -1;
-            else {
-                r.out = compact ? gacc++ : nacc[l]++;
-                SlotRec &pr = h.slots[sp][lp];
-                int c = 0; while (c < MAX_CHILD_REFS && pr.child[c] >= 0) c++;
-                if (c == MAX_CHILD_REFS) return -2;
-                pr.child[c] = (l << 8) | r.out;
-                pr.flags |= 1;
-            }
-        }
-    }
-    h.nacc = 0;
-    for (int l = 0; l < L; l++) h.nacc = std::max(h.nacc, nacc[l]);
-    if (compact) h.nacc = gacc;
-    return 0;
-}
-static int pick_lanes(const b2g_model *m, bool single) {
-    if (single) return 1;
-    int root_children = 0;
-    for (int i = 1; i < m->nl; i++) if (m->parent[i] == 0) root_children++;
-    const char *env = getenv("B2G_LANES");
-    if (env && (env[0] == '1' || env[0] == '2' || env[0] == '4' || env[0] == '8') && env[1] == 0) return env[0] - '0';
-    if (m->nl - 1 >= 16) return 4;                 // long trees (Humanoid, hands): chains run in parallel lanes
-    if (root_children >= 4) return 4;              // quadrupeds
-    if (root_children >= 2) return 2;
-    return 1;
-}
 
 static_assert(B2G_PLAN_MAX_SLOTS == MAX_SLOTS && B2G_PLAN_MAX_LANES == MAX_LANES, "plan table size");
 extern "C" int b2g_plan(const b2g_model *m, int32_t lanes, int32_t compact, int32_t *slots_out, int32_t info_out[5]) {
@@ -745,244 +656,38 @@ extern "C" int b2g_create(const b2g_model *m, const b2g_sim_params *sp, int32_t 
 extern "C" int b2g_create_ext(const b2g_model *m, const b2g_model_ext *ext, const b2g_sim_params *sp, int32_t num_envs, int32_t device,
                               b2g_sim **out) {
     if (!m || !sp || !out || num_envs <= 0) return fail(B2G_E_INVALID, "b2g_create: null argument or num_envs <= 0");
-    if (ext && (ext->actors_per_env < 1 || ext->obj_actor >= ext->actors_per_env || ext->obj_actor == 0 || ext->nbox < 0 ||
-                ext->nbox > MAX_BOX || ext->nten < 0 || ext->nten > MAX_TEN))
-        return fail(B2G_E_INVALID, "b2g_create_ext: bad actor / box / tendon counts");
-    if (ext && ext->obj_actor > 0 && sp->hf_samples) return fail(B2G_E_UNSUPPORTED, "b2g_create_ext: the free object needs the ground plane");
-    if (m->nl < 1 || m->nl > MAX_LINKS || m->nl - 1 > MAX_SLOTS || m->ncp > MAX_CP || m->nsens > MAX_SENS || m->nb > MAX_LINKS)
-        return fail(B2G_E_INVALID, "b2g_create: model exceeds compiled limits (links/contact points/sensors)");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
     if (ce != cudaSuccess || ndev == 0)
         return fail(B2G_E_CUDA, std::string("b2g_create: no CUDA device (there is no CPU fallback): ") + cudaGetErrorString(ce));
     CUDA_TRY(cudaSetDevice(device));
-    b2g_sim *s = new b2g_sim();
+    std::unique_ptr<b2g_sim> s(new b2g_sim());
     s->device = device; s->num_envs = num_envs;
-    memset(&s->buf, 0, sizeof(s->buf)); memset(s->buf_bytes, 0, sizeof(s->buf_bytes));
-    DevModel &h = s->hm;
-    memset(&h, 0, sizeof(h));
-    h.nl = m->nl; h.ncp = m->ncp; h.nb = m->nb; h.nsens = m->nsens;
-    h.root_fixed = m->root_fixed; h.gravity_on = m->gravity_on; h.substeps = sp->substeps;
-    h.h = sp->dt / (float)sp->substeps;
-    for (int c = 0; c < 3; c++) h.g[c] = m->gravity_on ? sp->gravity[c] : 0.f;
-    h.kn = m->contact_kn; h.cn = m->contact_cn; h.vs2 = m->contact_vs * m->contact_vs;
-    h.ground_mu = sp->ground_friction;
-    h.ang_damp = m->angular_damping; h.lin_damp = m->linear_damping; h.max_angvel = m->max_angular_velocity;
-    h.obj_ang_damp = ext ? ext->obj_angular_damping : 0.f; h.obj_lin_damp = ext ? ext->obj_linear_damping : 0.f;
-    // topology
-    const char *force1 = getenv("B2G_SINGLE_LANE");
-    const bool compact = ext && ext->obj_actor > 0;                     // [link][k][env] state layout (Stepper<.., OBJ>)
-    if (schedule(m, pick_lanes(m, force1 && force1[0] == '1'), h, compact) != 0) { delete s; return fail(B2G_E_INVALID, "b2g_create: the articulation does not fit the slot program limits"); }
-    s->lanes = h.lanes;
-    h.root_stride = ext ? ext->actors_per_env : 1;
-    h.obj_on = 0; h.obj_acc = h.obj_pose_acc = -1;
-    if (ext) {
-        if (ext->obj_actor > 0) {
-            h.obj_on = 1; h.obj_row = ext->obj_actor; h.obj_gravity_on = ext->obj_gravity_on;
-            h.obj_mass = ext->obj_mass; h.obj_kn = ext->obj_kn; h.obj_cn = ext->obj_cn; h.obj_mu = ext->obj_mu;
-            for (int c = 0; c < 3; c++) { h.obj_I[c] = ext->obj_inertia[c]; h.obj_half[c] = ext->obj_half[c]; }
-            h.obj_round = ext->obj_round; h.obj_max_angvel = ext->obj_max_angular_velocity;
-            if (ext->obj_round < 0.f || (ext->obj_round == 0.f && (ext->obj_half[0] <= 0.f || ext->obj_half[1] <= 0.f || ext->obj_half[2] <= 0.f))) {
-                delete s; return fail(B2G_E_INVALID, "b2g_create_ext: the object needs positive half extents, or a rounding radius");
-            }
-            h.obj_acc = h.nacc; h.obj_pose_acc = h.nacc + h.lanes; h.nacc += h.lanes + 1;   // env-wide ids: one sum per lane, one pose
-            // the object's gravity does not follow the articulation's disable_gravity flag (shadow_hand.py:239,279-282)
-            for (int c = 0; c < 3; c++) h.obj_g[c] = ext->obj_gravity_on ? sp->gravity[c] : 0.f;
-        }
-        h.nbox = ext->nbox;
-        for (int b = 0; b < ext->nbox; b++) {
-            h.box_link[b] = ext->box_link[b];
-            if (ext->box_link[b] < 0 || ext->box_link[b] >= m->nl) { delete s; return fail(B2G_E_INVALID, "b2g_create_ext: box link out of range"); }
-            const float *q = ext->box_quat[b];
-            float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
-            x /= n; y /= n; z /= n; w /= n;
-            const float R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                                2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                                2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-            memcpy(h.box_R[b], R, sizeof(R));
-            for (int c = 0; c < 3; c++) { h.box_pos[b][c] = ext->box_pos[b][c]; h.box_half[b][c] = ext->box_half[b][c]; }
-        }
-        h.nten = ext->nten; h.ten_k = ext->ten_k; h.ten_d = ext->ten_d;
-        for (int t = 0; t < ext->nten; t++) for (int k = 0; k < 2; k++) {
-            const int link = ext->ten_dof[t][k] + 1;
-            int ref = -1;
-            for (int sl = 0; sl < h.ns && ref < 0; sl++) for (int l = 0; l < h.lanes; l++) if (h.slots[sl][l].link == link) { ref = (l << 8) | sl; break; }
-            if (ref < 0) { delete s; return fail(B2G_E_INVALID, "b2g_create_ext: tendon joint index out of range"); }
-            h.ten_ref[t][k] = ref; h.ten_coef[t][k] = ext->ten_coef[t][k]; h.ten_range[t][k] = ext->ten_range[t][k];
-        }
-        if (h.nten > 0 && !h.obj_on) { delete s; return fail(B2G_E_UNSUPPORTED, "b2g_create_ext: tendons are only compiled into the object-enabled kernels"); }
-    }
-    if (compact) {
-        // per-env rows; one CTA = `blk / lanes` envs (+1 column of padding when that is even).  Prefer the CTA size that
-        // puts the most envs on an SM (registers: ~248 per thread in these kernels -> at most 256 threads per SM)
-        const size_t rows = (size_t)(h.nl - 1) * SLOT_F4 + (size_t)h.nacc * ACC_F4;
-        const size_t static_smem = sizeof(DevModel) + 64;
-        int best = 0; size_t best_envs = 0;
-        for (int blk : {128, 64, 32}) {
-            const int epb = blk / h.lanes;
-            if (epb < 1) continue;
-            const size_t bytes = rows * (size_t)(epb | 1) * sizeof(float4);
-            if (bytes + static_smem > 200 * 1024) continue;
-            const size_t ctas = std::min<size_t>((227 * 1024) / (bytes + static_smem + 1024), 256 / blk);
-            if (ctas * epb > best_envs) { best_envs = ctas * epb; best = blk; }
-        }
-        if (!best) { delete s; return fail(B2G_E_INVALID, "b2g_create: articulation too large for shared-memory slot state"); }
-        s->block = best; s->dyn_smem = rows * (size_t)((best / h.lanes) | 1) * sizeof(float4);
-    } else {   // CTA size: the per-thread slot state must fit in shared memory, preferably several CTAs per SM
-        const size_t per_thread = ((size_t)h.ns * SLOT_F4 + (size_t)h.nacc * ACC_F4) * sizeof(float4);
-        // self-collision scratch per ENV behind the accumulator pool: sphere centres, hit count, hit list (odd float4 count: banks)
-        h.self_on = (m->self_collide && m->self_pairs) ? 1 : 0;
-        h.self_f4 = 0;
-        if (h.self_on) {
-            // preferably in a run of consecutive slot cells of one lane that no link occupies (10 float4 each): no extra shared
-            // memory, the CTA size is unchanged
-            const int need = (m->ncp + 1 + SELF_HITS * 2 / 16 + SLOT_F4 - 1) / SLOT_F4;
-            int found = -1;
-            for (int l = 0; l < h.lanes && found < 0; l++) for (int s0 = 0; s0 + need <= h.ns && found < 0; s0++) {
-                bool idle = true;
-                for (int k = 0; k < need; k++) idle = idle && h.slots[s0 + k][l].link < 0;
-                if (idle) found = (l << 8) | s0;
-            }
-            h.self_cell = found;
-            if (found < 0 || getenv("B2G_SELF_APPENDED")) h.self_f4 = (m->ncp + 1 + SELF_HITS * 2 / 16) | 1;
-        }
-        auto bytes_of = [&](int b) { return per_thread * b + (size_t)(b / h.lanes) * h.self_f4 * sizeof(float4); };
-        int blk = 128;
-        const char *fb = getenv("B2G_BLOCK");                       // experiment hook: force a smaller CTA
-        if (fb && (atoi(fb) == 64 || atoi(fb) == 32)) blk = atoi(fb);
-        while (blk > 32 && bytes_of(blk) > 104 * 1024) blk >>= 1;
-        if (bytes_of(blk) > 200 * 1024) { delete s; return fail(B2G_E_INVALID, "b2g_create: articulation too large for shared-memory slot state"); }
-        s->block = blk; s->dyn_smem = bytes_of(blk);
-    }
-    // links
-    std::vector<int> order(m->ncp);
-    for (int i = 0; i < m->ncp; i++) order[i] = i;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return m->cp_link[a] < m->cp_link[b]; });
-    for (int i = 0; i < MAX_LINKS; i++) h.link_body[i] = -1;
-    for (int b = m->nb - 1; b >= 0; b--) { h.body_link[b] = m->body_link[b]; h.link_body[m->body_link[b]] = b; }
-    for (int b = 0; b < m->nb; b++) {
-        for (int c = 0; c < 3; c++) h.body_pos[b][c] = m->body_pos[3 * b + c];
-        for (int c = 0; c < 4; c++) h.body_quat[b][c] = m->body_quat[4 * b + c];
-    }
-    for (int i = 0; i < m->nl; i++) h.link_parent[i] = m->parent[i];
-    for (int k = 0; k < m->nsens; k++) {
-        h.sensor_body[k] = m->sensor_body[k];
-        for (int c = 0; c < 3; c++) h.sensor_bpos[k][c] = m->body_pos[3 * m->sensor_body[k] + c];
-    }
-    for (int i = 0; i < m->nl; i++) {
-        LinkC &l = h.links[i];
-        const float *q = m->lquat + 4 * i;
-        float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
-        x /= n; y /= n; z /= n; w /= n;
-        float R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                      2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                      2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-        memcpy(l.R0, R, sizeof(R));
-        for (int c = 0; c < 3; c++) { l.lpos[c] = m->lpos[3 * i + c]; l.axis[c] = m->axis[3 * i + c]; l.com[c] = m->com[3 * i + c]; }
-        for (int c = 0; c < 6; c++) l.Ic[c] = m->inertia[6 * i + c];
-        l.mass = m->mass[i];
-        l.armature = m->armature[i]; l.damping = m->damping[i]; l.stiffness = m->stiffness[i];
-        l.lower = m->lower[i]; l.upper = m->upper[i]; l.effort = m->effort[i];
-        l.kp = m->kp[i]; l.kd = m->kd[i]; l.limit_k = m->limit_k[i]; l.limit_d = m->limit_d[i];
-        {
-            const bool ident = fabsf(R[0] - 1.f) < 1e-7f && fabsf(R[4] - 1.f) < 1e-7f && fabsf(R[8] - 1.f) < 1e-7f;
-            l.flags = (m->jtype[i] == 1 ? LF_SLIDE : 0) | (m->limited[i] ? LF_LIMITED : 0) | (m->drive_mode[i] == 1 ? LF_POSDRIVE : 0) | (ident ? LF_R0_IDENTITY : 0);
-        }
-        l.sensor = -1;
-        l.cp_begin = l.cp_end = 0;
-    }
-    for (int k = 0; k < m->nsens; k++) h.links[m->body_link[m->sensor_body[k]]].sensor = k;
-    for (int k = 0; k < m->ncp; k++) {
-        int src = order[k];
-        CpC &c = h.cps[k];
-        for (int j = 0; j < 3; j++) c.pos[j] = m->cp_pos[3 * src + j];
-        c.radius = m->cp_radius[src]; c.mu = 0.5f * (m->cp_mu[src] + sp->ground_friction); c.body = m->cp_body[src]; c.pad = m->cp_link[src];
-        LinkC &l = h.links[m->cp_link[src]];
-        if (l.cp_end == 0 && l.cp_begin == 0) l.cp_begin = k;
-        l.cp_end = k + 1;
-    }
-    if (ext) for (int b = 0; b < ext->nbox; b++) h.links[ext->box_link[b]].flags |= LF_HAS_BOX;
-    {   // reach: bound on the distance of any contact sphere's far side from the root origin, over all joint positions
-        std::vector<float> dist(m->nl, 0.f);
-        for (int i = 1; i < m->nl; i++) {
-            const float *lp = m->lpos + 3 * i;
-            float d = sqrtf(lp[0] * lp[0] + lp[1] * lp[1] + lp[2] * lp[2]);
-            if (m->jtype[i] == 1) d += m->limited[i] ? std::max(fabsf(m->lower[i]), fabsf(m->upper[i])) : 1e30f;
-            dist[i] = dist[m->parent[i]] + d;
-        }
-        h.reach = 0.f;
-        for (int k = 0; k < m->ncp; k++) {
-            const float *cp = m->cp_pos + 3 * k;
-            h.reach = std::max(h.reach, dist[m->cp_link[k]] + sqrtf(cp[0] * cp[0] + cp[1] * cp[1] + cp[2] * cp[2]) + m->cp_radius[k]);
-        }
-    }
-    // self-collision tables (create_actor collision filter 0)
-    if (m->self_collide && m->self_pairs) {
-        if (compact || (ext && ext->obj_actor >= 0)) { delete s; return fail(B2G_E_UNSUPPORTED, "b2g_create_ext: self-collision is not compiled into the object-enabled kernels"); }
-        if (m->ncp > 64 || m->nl > MAX_LINKS) { delete s; return fail(B2G_E_UNSUPPORTED, "b2g_create: self-collision supports at most 64 contact spheres / 32 links"); }
-        h.self_kn = m->self_kn; h.self_cn = m->self_cn; h.self_mu = m->self_mu;
-        std::vector<int> inv(m->ncp);
-        for (int k = 0; k < m->ncp; k++) inv[order[k]] = k;
-        for (int i = 0; i < MAX_LINKS; i++) h.link_slot[i] = -1;
-        h.npairs = 0;
-        for (int a = 0; a < m->ncp; a++) for (int b = a + 1; b < m->ncp; b++) {
-            if (!m->self_pairs[(size_t)a * m->ncp + b] && !m->self_pairs[(size_t)b * m->ncp + a]) continue;
-            if (h.npairs >= MAX_PAIRS) { delete s; return fail(B2G_E_UNSUPPORTED, "b2g_create: too many self-collision pairs"); }
-            const int ia = std::min(inv[a], inv[b]), ib = std::max(inv[a], inv[b]);
-            h.pair_list[h.npairs++] = (unsigned short)(ia | (ib << 8));
-        }
-        while (h.npairs % (4 * h.lanes)) { if (h.npairs >= MAX_PAIRS) { delete s; return fail(B2G_E_UNSUPPORTED, "b2g_create: too many self-collision pairs"); } h.pair_list[h.npairs++] = 0; }
-        h.npairs /= 4;                                              // quads from here on
-        for (int sl = 0; sl < h.ns; sl++) for (int l = 0; l < h.lanes; l++) if (h.slots[sl][l].link > 0) h.link_slot[h.slots[sl][l].link] = (l << 8) | sl;
-    }
-    // height field
+    // the reference paths the tests compare with: B2G_SINGLE_LANE=1 one thread per env, B2G_NO_QUAD=1 the generic Stepper
+    const char *single = getenv("B2G_SINGLE_LANE"), *no_quad = getenv("B2G_NO_QUAD");
+    const char *err = "";
+    const int rc = build_sim_model(m, ext, sp, single && single[0] == '1', no_quad && no_quad[0] == '1', *s, &err);
+    if (rc != B2G_OK) return fail(rc, err);
     if (sp->hf_samples) {
-        h.has_hf = 1; h.hf_nx = sp->hf_nx; h.hf_ny = sp->hf_ny;
-        h.hf_scale = sp->hf_horizontal_scale; h.hf_inv_scale = 1.f / sp->hf_horizontal_scale; h.hf_vscale = sp->hf_vertical_scale;
-        h.hf_ox = sp->hf_origin_x; h.hf_oy = sp->hf_origin_y;
-        size_t bytes = (size_t)sp->hf_nx * sp->hf_ny * sizeof(int16_t);
+        const size_t bytes = (size_t)sp->hf_nx * sp->hf_ny * sizeof(int16_t);
         CUDA_TRY(cudaMalloc(&s->d_hf, bytes));
         CUDA_TRY(cudaMemcpy(s->d_hf, sp->hf_samples, bytes, cudaMemcpyHostToDevice));
     }
     CUDA_TRY(cudaMalloc(&s->dm, sizeof(DevModel)));
-    CUDA_TRY(cudaMemcpy(s->dm, &h, sizeof(DevModel), cudaMemcpyHostToDevice));
-    s->kin_ok = kin_build(m, h.root_stride, s->hk) == 0;
+    CUDA_TRY(cudaMemcpy(s->dm, &s->hm, sizeof(DevModel), cudaMemcpyHostToDevice));
     if (s->kin_ok) {
         CUDA_TRY(cudaMalloc(&s->d_kin, sizeof(KinModel)));
         CUDA_TRY(cudaMemcpy(s->d_kin, &s->hk, sizeof(KinModel), cudaMemcpyHostToDevice));
     }
-    {   // the specialised path of "four hinge chains on a free base" (Ant, ANYmal): b2g_quad.cuh
-        const char *nq = getenv("B2G_NO_QUAD"), *qb = getenv("B2G_QUAD_BLOCK"), *nz = getenv("B2G_NO_ZERO_COPY");
-        s->no_zero_copy = nz != nullptr;
-        if (const char *hc = getenv("B2G_HOSTIO_CTAS")) {      // experiment hook: resident CTAs per SM of the host-I/O Ant step (2..6)
-            const int c = atoi(hc);
-            if (c >= 2 && c <= 6) s->hostio_pad = (size_t)(227 * 1024 / c - 1024 - 32 * 1024) & ~(size_t)15;
-        }
-        if (qb && (atoi(qb) == 32 || atoi(qb) == 64 || atoi(qb) == 128)) s->quad_block = atoi(qb);
-        if (!(nq && nq[0] == '1') && !ext && !h.self_on && !(force1 && force1[0] == '1') && !getenv("B2G_LANES") && !getenv("B2G_BLOCK")) {
-            std::vector<float> qm; int leg_link[12], spec = 0;
-            const char *nsp = getenv("B2G_QUAD_NO_SPEC");
-            const int ns = quad_build(m, sp, qm, leg_link, &spec, (nsp && nsp[0] == '1') ? 0 : 3);
-            s->quad_spec = spec;
-            if (ns) {
-                CUDA_TRY(cudaMalloc(&s->d_qm, qm.size() * sizeof(float)));
-                CUDA_TRY(cudaMemcpy(s->d_qm, qm.data(), qm.size() * sizeof(float), cudaMemcpyHostToDevice));
-                s->quad_ns = ns;
-            }
-        }
+    if (s->quad_ns) {
+        CUDA_TRY(cudaMalloc(&s->d_qm, s->qm.size() * sizeof(float)));
+        CUDA_TRY(cudaMemcpy(s->d_qm, s->qm.data(), s->qm.size() * sizeof(float), cudaMemcpyHostToDevice));
     }
-    *out = s;
+    *out = s.release();
     return B2G_OK;
 }
 
 extern "C" int b2g_destroy(b2g_sim *s) {
-    if (!s) return B2G_OK;
-    cudaSetDevice(s->device);
-    if (s->dm) cudaFree(s->dm);
-    if (s->d_hf) cudaFree(s->d_hf);
-    if (s->d_actions_stage) cudaFree(s->d_actions_stage);
-    if (s->d_qm) cudaFree(s->d_qm);
-    if (s->d_kin) cudaFree(s->d_kin);
     delete s;
     return B2G_OK;
 }
@@ -1021,19 +726,24 @@ extern "C" int b2g_bind(b2g_sim *s, int32_t slot, void *ptr, size_t bytes) {
     return B2G_OK;
 }
 
-// developer switches read once per process (never on the step path)
-static bool getenv_once(const char *name) {
-    static std::vector<std::pair<std::string, bool>> cache;
-    for (auto &kv : cache) if (kv.first == name) return kv.second;
-    const char *v = getenv(name);
-    cache.emplace_back(name, v && v[0] == '1');
-    return cache.back().second;
-}
-
 static int require(const b2g_sim *s, std::initializer_list<int> slots, const char *who) {
     for (int k : slots) if (!s->buf.p[k]) return fail(B2G_E_UNBOUND, std::string(who) + ": tensor slot " + std::to_string(k) + " is not bound");
     return B2G_OK;
 }
+
+// the action and observation counts of the task set on the sim
+static void task_sizes(const b2g_sim *s, int *n_act, int *n_obs) {
+    if (s->has_anymal) { *n_act = s->anymal.num_actions; *n_obs = s->anymal.num_obs; }
+    else if (s->has_hand) { *n_act = s->hand.num_actions; *n_obs = s->hand.num_obs; }
+    else { *n_act = s->task.num_actions; *n_obs = s->task.num_obs; }
+}
+
+// Whole tiles for the bulk-copy step kernels: the envs fill whole CTAs of `epb`, and every per-env tile of a CTA, down to
+// the one-byte time-out flags, is a whole number of 16-byte units (epb % 16 == 0 covers every wider row as well)
+static bool whole_tiles(size_t N, int epb) { return N % epb == 0 && epb % 16 == 0; }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// launches
 
 // raise a kernel's dynamic shared-memory limit, once per (sim, kernel): the attribute call costs microseconds of host
 // time, comparable to a whole step when issued before every launch
@@ -1045,74 +755,104 @@ static int set_smem(b2g_sim *s, K kernel, size_t bytes) {
     s->smem_set.push_back(key);
     return B2G_OK;
 }
-#define B2G_LAUNCH(KERNEL, ...)                                                                  \
-    do {                                                                                          \
-        int rc_ = set_smem(s, KERNEL, s->dyn_smem); if (rc_) return rc_;                          \
-        KERNEL<<<grid, blk, s->dyn_smem, st>>>(__VA_ARGS__);                                      \
-    } while (0)
-// dispatch on (lanes, height field, CTA size)
-#define B2G_DISPATCH_LHB(NAME, ...)                                                                                   \
-    do {                                                                                                               \
-        const bool hf_ = s->d_hf != nullptr;                                                                           \
-        if (s->lanes == 4 && !hf_ && blk == 128) B2G_LAUNCH((NAME<4, false, 128>), __VA_ARGS__);                       \
-        else if (s->lanes == 4 && hf_ && blk == 128) B2G_LAUNCH((NAME<4, true, 128>), __VA_ARGS__);                    \
-        else if (s->lanes == 4 && !hf_ && blk == 64) B2G_LAUNCH((NAME<4, false, 64>), __VA_ARGS__);                    \
-        else if (s->lanes == 4 && !hf_ && blk == 32) B2G_LAUNCH((NAME<4, false, 32>), __VA_ARGS__);                    \
-        else if (s->lanes == 2 && !hf_ && blk == 128) B2G_LAUNCH((NAME<2, false, 128>), __VA_ARGS__);                  \
-        else if (s->lanes == 2 && !hf_ && blk == 64) B2G_LAUNCH((NAME<2, false, 64>), __VA_ARGS__);                    \
-        else if (s->lanes == 2 && !hf_ && blk == 32) B2G_LAUNCH((NAME<2, false, 32>), __VA_ARGS__);                    \
-        else if (s->lanes == 1 && !hf_ && blk == 128) B2G_LAUNCH((NAME<1, false, 128>), __VA_ARGS__);                  \
-        else if (s->lanes == 1 && !hf_ && blk == 64) B2G_LAUNCH((NAME<1, false, 64>), __VA_ARGS__);                    \
-        else if (s->lanes == 1 && !hf_ && blk == 32) B2G_LAUNCH((NAME<1, false, 32>), __VA_ARGS__);                    \
-        else return fail(B2G_E_UNSUPPORTED, "no kernel instantiated for this (lanes, terrain, CTA size) combination"); \
-    } while (0)
+
+// PLAIN: as is.  SMEM: raise the kernel's dynamic shared-memory limit first (set_smem; the attribute can also change the
+// shared-memory carveout, so only the kernels that size their shared memory at run time ask for it).  SMEM_PDL: and let the
+// grid start while the previous kernel in the stream drains (programmatic dependent launch: the kernel's griddepcontrol.wait).
+enum LaunchMode { PLAIN, SMEM, SMEM_PDL };
+
+template <typename... P, typename... A>
+static int launch(b2g_sim *s, void (*kernel)(P...), int grid, int block, size_t dyn, cudaStream_t st, LaunchMode mode, A... args) {
+    if (mode != PLAIN) { const int rc = set_smem(s, kernel, dyn); if (rc) return rc; }
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3(grid); lc.blockDim = dim3(block); lc.dynamicSmemBytes = dyn; lc.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    if (mode == SMEM_PDL) { lc.attrs = at; lc.numAttrs = 1; }
+    CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, args...));
+    s->launches++;
+    CUDA_TRY(cudaGetLastError());
+    return B2G_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Instantiation lists: one function per kernel family maps the runtime key to the compiled instantiation, null when there
+// is none; every instantiation the library contains is listed once.  The kernels are compiled in the order they are first
+// named, so the lists keep the order the entry points have always named them in: quad simulate, simulate, (Jacobian),
+// ShadowHand, AnymalTerrain, (Cartpole), quad locomotion, locomotion, (rollout).
+static constexpr int key(int lanes, int block) { return (lanes << 8) | block; }
+
+// gym.simulate() on the quad sub-step: (chain length, height field, specialisation); 128 threads, one env per 4
+constexpr int QUAD_SIM_BLOCK = 128;
+using QuadSimKernel = void (*)(const float4 *, const int16_t *, Buffers, int, int);
+static QuadSimKernel quad_simulate_kernel_for(int ns, bool hf, int spec) {
+    constexpr int B = QUAD_SIM_BLOCK;
+    const bool sp3 = spec == 3;
+    if (ns == 2 && !hf) return sp3 ? quad_simulate_kernel<2, false, 3, B> : quad_simulate_kernel<2, false, 0, B>;
+    if (ns == 2) return sp3 ? quad_simulate_kernel<2, true, 3, B> : quad_simulate_kernel<2, true, 0, B>;
+    if (ns == 3 && !hf) return sp3 ? quad_simulate_kernel<3, false, 3, B> : quad_simulate_kernel<3, false, 0, B>;
+    if (ns == 3) return sp3 ? quad_simulate_kernel<3, true, 3, B> : quad_simulate_kernel<3, true, 0, B>;
+    return nullptr;
+}
+
+// gym.simulate() on the generic Stepper: (lanes, CTA size, height field, free object, self-collision)
+using SimulateKernel = void (*)(const DevModel *, const int16_t *, Buffers, int);
+static SimulateKernel simulate_kernel_for(int lanes, int block, bool hf, bool obj, bool self) {
+    if (obj) {                   // the free object (b2g_create_ext keeps it on the ground plane)
+        switch (key(lanes, block)) {
+            case key(8, 128): return simulate_kernel<8, false, 128, true>;
+            case key(8, 64): return simulate_kernel<8, false, 64, true>;
+            case key(4, 128): return simulate_kernel<4, false, 128, true>;
+            case key(4, 64): return simulate_kernel<4, false, 64, true>;
+            case key(4, 32): return simulate_kernel<4, false, 32, true>;
+            case key(1, 32): return simulate_kernel<1, false, 32, true>;
+        }
+        return nullptr;
+    }
+    if (self) {                  // link-link contact, on the ground plane
+        if (hf) return nullptr;
+        switch (key(lanes, block)) {
+            case key(4, 128): return simulate_kernel<4, false, 128, false, true>;
+            case key(4, 64): return simulate_kernel<4, false, 64, false, true>;
+            case key(4, 32): return simulate_kernel<4, false, 32, false, true>;
+            case key(1, 64): return simulate_kernel<1, false, 64, false, true>;
+            case key(1, 32): return simulate_kernel<1, false, 32, false, true>;
+        }
+        return nullptr;
+    }
+    if (hf && key(lanes, block) != key(4, 128)) return nullptr;          // the height field: 4 lanes, 128 threads
+    switch (key(lanes, block)) {
+        case key(4, 128): return !hf ? simulate_kernel<4, false, 128> : simulate_kernel<4, true, 128>;
+        case key(4, 64): return simulate_kernel<4, false, 64>;
+        case key(4, 32): return simulate_kernel<4, false, 32>;
+        case key(2, 128): return simulate_kernel<2, false, 128>;
+        case key(2, 64): return simulate_kernel<2, false, 64>;
+        case key(2, 32): return simulate_kernel<2, false, 32>;
+        case key(1, 128): return simulate_kernel<1, false, 128>;
+        case key(1, 64): return simulate_kernel<1, false, 64>;
+        case key(1, 32): return simulate_kernel<1, false, 32>;
+    }
+    return nullptr;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 
 extern "C" int b2g_simulate(b2g_sim *s, void *stream) {
     if (!s) return fail(B2G_E_INVALID, "b2g_simulate: null sim");
     int rc = require(s, {B2G_T_ROOT_STATE, B2G_T_DOF_STATE}, "b2g_simulate"); if (rc) return rc;
     CUDA_TRY(cudaSetDevice(s->device));
     cudaStream_t st = (cudaStream_t)stream;
+    const int N = s->num_envs;
     if (s->quad_ns) {
-        constexpr int QB = 128;
-        const int N = s->num_envs, grid = (N * 4 + QB - 1) / QB;
-        const size_t dyn = ((size_t)quad_park_f4(s->quad_ns) * QB + quad_model_f4(s->quad_ns)) * sizeof(float4);
-#define QSIM(NS_, HF_, SP_)                                                                                         \
-        do {                                                                                                        \
-            int rc_ = set_smem(s, quad_simulate_kernel<NS_, HF_, SP_, QB>, dyn); if (rc_) return rc_;               \
-            quad_simulate_kernel<NS_, HF_, SP_, QB><<<grid, QB, dyn, st>>>(s->d_qm, s->d_hf, s->buf, N, s->hm.substeps); \
-        } while (0)
-        const bool sp3 = s->quad_spec == 3;
-        if (s->quad_ns == 2 && !s->d_hf) { if (sp3) QSIM(2, false, 3); else QSIM(2, false, 0); }
-        else if (s->quad_ns == 2) { if (sp3) QSIM(2, true, 3); else QSIM(2, true, 0); }
-        else if (s->quad_ns == 3 && !s->d_hf) { if (sp3) QSIM(3, false, 3); else QSIM(3, false, 0); }
-        else { if (sp3) QSIM(3, true, 3); else QSIM(3, true, 0); }
-#undef QSIM
-        s->launches++;
-        CUDA_TRY(cudaGetLastError());
-        return B2G_OK;
+        const size_t dyn = ((size_t)quad_park_f4(s->quad_ns) * QUAD_SIM_BLOCK + quad_model_f4(s->quad_ns)) * sizeof(float4);
+        return launch(s, quad_simulate_kernel_for(s->quad_ns, s->d_hf != nullptr, s->quad_spec), (N * 4 + QUAD_SIM_BLOCK - 1) / QUAD_SIM_BLOCK,
+                      QUAD_SIM_BLOCK, dyn, st, SMEM, s->d_qm, s->d_hf, s->buf, N, s->hm.substeps);
     }
-    const int N = s->num_envs, blk = s->block, grid = (N * s->lanes + blk - 1) / blk;
-    if (s->hm.obj_on) {
-        if (s->lanes == 8 && blk == 128) B2G_LAUNCH((simulate_kernel<8, false, 128, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 8 && blk == 64) B2G_LAUNCH((simulate_kernel<8, false, 64, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 4 && blk == 128) B2G_LAUNCH((simulate_kernel<4, false, 128, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 4 && blk == 64) B2G_LAUNCH((simulate_kernel<4, false, 64, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 4 && blk == 32) B2G_LAUNCH((simulate_kernel<4, false, 32, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 1 && blk == 32) B2G_LAUNCH((simulate_kernel<1, false, 32, true>), s->dm, s->d_hf, s->buf, N);
-        else return fail(B2G_E_UNSUPPORTED, "no object-enabled kernel instantiated for this (lanes, CTA size) combination");
-    } else if (s->hm.self_on) {      // link-link contact: its own instantiations
-        if (s->d_hf) return fail(B2G_E_UNSUPPORTED, "self-collision kernels are instantiated for the ground plane");
-        if (s->lanes == 4 && blk == 128) B2G_LAUNCH((simulate_kernel<4, false, 128, false, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 4 && blk == 64) B2G_LAUNCH((simulate_kernel<4, false, 64, false, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 4 && blk == 32) B2G_LAUNCH((simulate_kernel<4, false, 32, false, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 1 && blk == 64) B2G_LAUNCH((simulate_kernel<1, false, 64, false, true>), s->dm, s->d_hf, s->buf, N);
-        else if (s->lanes == 1 && blk == 32) B2G_LAUNCH((simulate_kernel<1, false, 32, false, true>), s->dm, s->d_hf, s->buf, N);
-        else return fail(B2G_E_UNSUPPORTED, "no self-collision kernel instantiated for this (lanes, CTA size) combination");
-    } else
-        B2G_DISPATCH_LHB(simulate_kernel, s->dm, s->d_hf, s->buf, N);
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    const int blk = s->block, grid = (N * s->lanes + blk - 1) / blk;
+    const SimulateKernel k = simulate_kernel_for(s->lanes, blk, s->d_hf != nullptr, s->hm.obj_on, s->hm.self_on);
+    if (!k) return fail(B2G_E_UNSUPPORTED, "no simulate kernel instantiated for this (lanes, CTA size, terrain, free object, self-collision) combination");
+    return launch(s, k, grid, blk, s->dyn_smem, st, SMEM, s->dm, s->d_hf, s->buf, N);
 }
 
 extern "C" int b2g_refresh_rigid_body_state(b2g_sim *s, void *stream) {
@@ -1120,10 +860,7 @@ extern "C" int b2g_refresh_rigid_body_state(b2g_sim *s, void *stream) {
     int rc = require(s, {B2G_T_ROOT_STATE, B2G_T_DOF_STATE, B2G_T_RIGID_BODY_STATE}, "b2g_refresh_rigid_body_state"); if (rc) return rc;
     CUDA_TRY(cudaSetDevice(s->device));
     const int N = s->num_envs;
-    body_state_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(s->dm, s->buf, N);
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    return launch(s, body_state_kernel, (N + 127) / 128, 128, 0, (cudaStream_t)stream, PLAIN, s->dm, s->buf, N);
 }
 
 extern "C" int b2g_kin_shape(const b2g_sim *s, int32_t shape_out[2]) {
@@ -1150,16 +887,12 @@ extern "C" int b2g_refresh_kinematic_tensors(b2g_sim *s, int32_t which, void *st
     // CTAs, the warps stride over the envs
     int sms = 0;
     CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device));
-    if (s->hk.nl <= 16 && s->hk.nb <= 16) {
-        const int grid = std::min((N + 2 * WARPS - 1) / (2 * WARPS), sms * 8);
-        kin_tensors_kernel<WARPS, 16><<<grid, WARPS * 32, 0, (cudaStream_t)stream>>>(s->d_kin, root, dof, J, M, N);
-    } else {
-        const int grid = std::min((N + WARPS - 1) / WARPS, sms * 8);
-        kin_tensors_kernel<WARPS, 32><<<grid, WARPS * 32, 0, (cudaStream_t)stream>>>(s->d_kin, root, dof, J, M, N);
-    }
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (s->hk.nl <= 16 && s->hk.nb <= 16)
+        return launch(s, kin_tensors_kernel<WARPS, 16>, std::min((N + 2 * WARPS - 1) / (2 * WARPS), sms * 8), WARPS * 32, 0, st, PLAIN,
+                      s->d_kin, root, dof, J, M, N);
+    return launch(s, kin_tensors_kernel<WARPS, 32>, std::min((N + WARPS - 1) / WARPS, sms * 8), WARPS * 32, 0, st, PLAIN,
+                  s->d_kin, root, dof, J, M, N);
 }
 
 extern "C" int b2g_set_task(b2g_sim *s, const b2g_task_params *t) {
@@ -1207,19 +940,11 @@ extern "C" int b2g_set_hand_task(b2g_sim *s, const b2g_hand_params *t) {
     for (int f = 0; f < 5; f++) {
         const int b = t->fingertip_body[f];
         if (b < 0 || b >= h.nb || h.sensor_body[f] != b) return fail(B2G_E_INVALID, "ShadowHand: fingertip bodies must be the five force-sensor bodies, in order");
-        const int link = h.body_link[b];
-        int ref = -1;
-        for (int sl = 0; sl < h.ns && ref < 0; sl++) for (int l = 0; l < h.lanes; l++) if (h.slots[sl][l].link == link) { ref = (l << 8) | sl; break; }
+        const int ref = slot_of_link(h, h.body_link[b]);
         if (ref < 0) return fail(B2G_E_UNSUPPORTED, "ShadowHand: a fingertip rides on the root link");
         H.ft_ref[f] = ref;
         for (int c = 0; c < 3; c++) H.ft_bpos[f][c] = h.body_pos[b][c];
-        const float *q = h.body_quat[b];
-        float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
-        x /= n; y /= n; z /= n; w /= n;
-        const float R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                            2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                            2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-        memcpy(H.ft_bR[f], R, sizeof(R));
+        host_quat_to_mat(h.body_quat[b], H.ft_bR[f]);
     }
     // observation layouts, shadow_hand.py:460-592
     const int A = t->num_actions;
@@ -1247,6 +972,20 @@ extern "C" int b2g_set_hand_task(b2g_sim *s, const b2g_hand_params *t) {
     return B2G_OK;
 }
 
+// the fused ShadowHand step: (lanes, CTA size)
+using HandKernel = void (*)(const DevModel *, Buffers, b2g_hand_params, HandDev, const float *, int);
+static HandKernel hand_kernel_for(int lanes, int block) {
+    switch (key(lanes, block)) {
+        case key(8, 128): return hand_step_kernel<8, 128>;
+        case key(8, 64): return hand_step_kernel<8, 64>;
+        case key(4, 128): return hand_step_kernel<4, 128>;
+        case key(4, 64): return hand_step_kernel<4, 64>;
+        case key(4, 32): return hand_step_kernel<4, 32>;
+        case key(1, 32): return hand_step_kernel<1, 32>;
+    }
+    return nullptr;
+}
+
 static int hand_step(b2g_sim *s, const float *actions, void *stream) {
     const b2g_hand_params &P = s->hand;
     int rc = require(s, {B2G_T_ROOT_STATE, B2G_T_DOF_STATE, B2G_T_DOF_TARGET, B2G_T_OBS, B2G_T_REW, B2G_T_RESET, B2G_T_PROGRESS, B2G_T_RESET_COUNT,
@@ -1262,18 +1001,24 @@ static int hand_step(b2g_sim *s, const float *actions, void *stream) {
     const size_t N = s->num_envs;
     if (s->buf_bytes[B2G_T_OBS] < N * P.num_obs * 4) return fail(B2G_E_INVALID, "OBS buffer too small");
     CUDA_TRY(cudaSetDevice(s->device));
-    cudaStream_t st = (cudaStream_t)stream;
     const int blk = s->block, grid = ((int)N * s->lanes + blk - 1) / blk;
-    if (s->lanes == 8 && blk == 128) B2G_LAUNCH((hand_step_kernel<8, 128>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else if (s->lanes == 8 && blk == 64) B2G_LAUNCH((hand_step_kernel<8, 64>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else if (s->lanes == 4 && blk == 128) B2G_LAUNCH((hand_step_kernel<4, 128>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else if (s->lanes == 4 && blk == 64) B2G_LAUNCH((hand_step_kernel<4, 64>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else if (s->lanes == 4 && blk == 32) B2G_LAUNCH((hand_step_kernel<4, 32>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else if (s->lanes == 1 && blk == 32) B2G_LAUNCH((hand_step_kernel<1, 32>), s->dm, s->buf, P, s->hand_dev, actions, (int)N);
-    else return fail(B2G_E_UNSUPPORTED, "no ShadowHand kernel instantiated for this (lanes, CTA size) combination");
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    const HandKernel k = hand_kernel_for(s->lanes, blk);
+    if (!k) return fail(B2G_E_UNSUPPORTED, "no ShadowHand kernel instantiated for this (lanes, CTA size) combination");
+    return launch(s, k, grid, blk, s->dyn_smem, (cudaStream_t)stream, SMEM, s->dm, s->buf, P, s->hand_dev, actions, (int)N);
+}
+
+// AnymalTerrain physics (the first of its two kernels): the quad sub-step when the model is on the quad path (on a height
+// field with or without per-env physical parameters), else the generic Stepper; plane or height field.  128 threads.
+static int launch_anymal_physics(b2g_sim *s, const b2g_anymal_params &P, const float *actions, int N, int grid, cudaStream_t st) {
+    const bool hf = s->d_hf != nullptr;
+    if (s->quad_ns == 3) {
+        const bool dr = s->buf.p[B2G_T_ENV_MASS_SCALE] || s->buf.p[B2G_T_ENV_DOF_PROPS];
+        const auto k = hf ? (dr ? quad_anymal_physics_kernel<true, 128, true> : quad_anymal_physics_kernel<true, 128, false>) : quad_anymal_physics_kernel<false, 128>;
+        const size_t dyn = ((size_t)quad_park_f4(3) * 128 + quad_model_f4(3)) * sizeof(float4);
+        return launch(s, k, grid, 128, dyn, st, SMEM, s->d_qm, s->d_hf, s->buf, P, actions, N, s->hm.substeps, s->step_counter);
+    }
+    const auto k = hf ? anymal_physics_kernel<4, true, 128> : anymal_physics_kernel<4, false, 128>;
+    return launch(s, k, grid, 128, s->dyn_smem, st, SMEM, s->dm, s->d_hf, s->buf, P, actions, N, s->step_counter);
 }
 
 static int anymal_step(b2g_sim *s, const float *actions, void *stream) {
@@ -1286,42 +1031,43 @@ static int anymal_step(b2g_sim *s, const float *actions, void *stream) {
     if (P.custom_origins) { rc = require(s, {B2G_T_ENV_ORIGINS, B2G_T_TERRAIN_LEVELS, B2G_T_TERRAIN_TYPES, B2G_T_TERRAIN_ORIGINS}, "b2g_task_step(AnymalTerrain)"); if (rc) return rc; }
     CUDA_TRY(cudaSetDevice(s->device));
     cudaStream_t st = (cudaStream_t)stream;
-    const int N = s->num_envs, blk = 128, grid = (N * 4 + blk - 1) / blk;
+    const int N = s->num_envs, grid = (N * 4 + 127) / 128;
     if (s->block != 128) return fail(B2G_E_UNSUPPORTED, "AnymalTerrain: unexpected CTA size");
     if (grid > REDUCE_PARTIALS) return fail(B2G_E_INVALID, "AnymalTerrain: too many blocks for the reduction scratch (num_envs <= 32768)");
     if (s->buf_bytes[B2G_T_REDUCE_SCRATCH] < (REDUCE_PARTIALS + 48) * 4) return fail(B2G_E_INVALID, "REDUCE_SCRATCH too small");
     s->step_counter++;                                   // common_step_counter += 1 (:459) before the push test
-    if (s->quad_ns == 3) {                               // the specialised sub-step (b2g_quad.cuh), joint state in registers
-        const size_t dyn = ((size_t)quad_park_f4(3) * 128 + quad_model_f4(3)) * sizeof(float4);
-        if (s->d_hf) {
-            const bool dr = s->buf.p[B2G_T_ENV_MASS_SCALE] || s->buf.p[B2G_T_ENV_DOF_PROPS];
-            if (dr) {
-                rc = set_smem(s, quad_anymal_physics_kernel<true, 128, true>, dyn); if (rc) return rc;
-                quad_anymal_physics_kernel<true, 128, true><<<grid, blk, dyn, st>>>(s->d_qm, s->d_hf, s->buf, P, actions, N, s->hm.substeps, s->step_counter);
-            } else {
-                rc = set_smem(s, quad_anymal_physics_kernel<true, 128, false>, dyn); if (rc) return rc;
-                quad_anymal_physics_kernel<true, 128, false><<<grid, blk, dyn, st>>>(s->d_qm, s->d_hf, s->buf, P, actions, N, s->hm.substeps, s->step_counter);
-            }
-        } else {
-            rc = set_smem(s, quad_anymal_physics_kernel<false, 128>, dyn); if (rc) return rc;
-            quad_anymal_physics_kernel<false, 128><<<grid, blk, dyn, st>>>(s->d_qm, s->d_hf, s->buf, P, actions, N, s->hm.substeps, s->step_counter);
-        }
-    } else if (s->d_hf) {
-        rc = set_smem(s, anymal_physics_kernel<4, true, 128>, s->dyn_smem); if (rc) return rc;
-        anymal_physics_kernel<4, true, 128><<<grid, blk, s->dyn_smem, st>>>(s->dm, s->d_hf, s->buf, P, actions, N, s->step_counter);
-    } else {
-        rc = set_smem(s, anymal_physics_kernel<4, false, 128>, s->dyn_smem); if (rc) return rc;
-        anymal_physics_kernel<4, false, 128><<<grid, blk, s->dyn_smem, st>>>(s->dm, s->d_hf, s->buf, P, actions, N, s->step_counter);
-    }
+    rc = launch_anymal_physics(s, P, actions, N, grid, st); if (rc) return rc;
     // kernel 2: one WARP per env -- the 140-point height gather (anymal_terrain.py:515-538) and the 188 observation
     // stores dominate it; with 4 lanes per env the 4096-env workload was 512 warps on 592 schedulers
-    anymal_reset_obs_kernel<32, 128><<<(N * 32 + 127) / 128, 128, 0, st>>>(s->buf, P, s->d_hf, N, s->hm.nl - 1, grid, s->step_counter, 0);
-    s->launches += 2;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    return launch(s, anymal_reset_obs_kernel<32, 128>, (N * 32 + 127) / 128, 128, 0, st, PLAIN,
+                  s->buf, P, s->d_hf, N, s->hm.nl - 1, grid, s->step_counter, 0);
 }
 
-extern "C" int b2g_task_step(b2g_sim *s, const float *actions, void *stream) {
+// b2g_task_step_host with pinned host buffers: the step kernel reads its actions from host memory and writes what
+// VecTask.step returns straight to these buffers
+struct HostOut {
+    float *obs, *rew;
+    long long *reset;
+    uint8_t *timeout;
+};
+
+static TileArgs tile_args(bool on, size_t io_bytes_at, size_t model_bytes_at, const float *actions, const HostOut *io) {
+    TileArgs ta;
+    ta.on = on ? 1 : 0; ta.io_f4 = (int)(io_bytes_at / 16); ta.model_f4 = (int)(model_bytes_at / 16);
+    ta.h_act = io ? actions : nullptr;
+    ta.h_obs = io ? io->obs : nullptr; ta.h_rew = io ? io->rew : nullptr; ta.h_reset = io ? io->reset : nullptr; ta.h_timeout = io ? io->timeout : nullptr;
+    return ta;
+}
+
+// the locomotion step lists, defined behind task_step (see "Instantiation lists")
+constexpr int QUAD_LOCO_BLOCK = 64;
+using QuadLocoKernel = void (*)(const float4 *, Buffers, b2g_task_params, const float *, int, int, TileArgs);
+using LocoKernel = void (*)(const DevModel *, const int16_t *, Buffers, b2g_task_params, const float *, int, TileArgs);
+static QuadLocoKernel quad_loco_kernel_for(int spec, bool hostio, bool lean);
+static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self);
+
+// One VecTask.step(); io: the pinned host buffers the Ant / Humanoid step kernel writes to itself (null: device I/O)
+static int task_step(b2g_sim *s, const float *actions, void *stream, const HostOut *io) {
     if (!s || !actions) return fail(B2G_E_INVALID, "b2g_task_step: null argument");
     if (s->has_anymal) return anymal_step(s, actions, stream);
     if (s->has_hand) return hand_step(s, actions, stream);
@@ -1337,126 +1083,87 @@ extern "C" int b2g_task_step(b2g_sim *s, const float *actions, void *stream) {
     const int blk = s->block, grid = ((int)N * s->lanes + blk - 1) / blk;
     if (P.task == B2G_TASK_CARTPOLE) {
         if (blk != 128) return fail(B2G_E_UNSUPPORTED, "cartpole: unexpected CTA size");
-        B2G_LAUNCH((cartpole_step_kernel<128>), s->dm, s->buf, P, actions, (int)N);
-    } else {
-        rc = require(s, {B2G_T_POTENTIALS, B2G_T_PREV_POTENTIALS, B2G_T_INITIAL_ROOT}, "b2g_task_step"); if (rc) return rc;
-        const bool hum = P.task == B2G_TASK_HUMANOID;
-        if (!hum && s->quad_ns == 2 && !s->d_hf) {           // Ant on the quad sub-step (whole tiles only)
-            const int qb = s->quad_block, epb = qb / 4, nd_ = 8, O = P.num_obs, ns6 = 6 * s->hm.nsens;
-            const bool clip_sep = s->buf.p[B2G_T_OBS_CLIPPED] && s->buf.p[B2G_T_OBS_CLIPPED] != s->buf.p[B2G_T_OBS];
-            const size_t park_bytes = (size_t)quad_park_f4(2) * qb * sizeof(float4);
-            const size_t io_bytes = ((size_t)epb * (13 + 3 * nd_ + ns6) * 4 + 15) & ~(size_t)15;
-            const size_t out_bytes = (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1);
-            const bool ok = (N % epb == 0) && ((epb * ns6 * 4) % 16 == 0) && ((epb * O * 4) % 16 == 0) && out_bytes <= park_bytes;
-            if (ok) {
-                // Host-I/O launches ask for more shared memory than they use: fewer CTAs are resident, the grid runs in several waves,
-                // and a later wave computes while the PCIe writes of an earlier one drain (all CTAs of a single wave reach their
-                // store phase together and the link idles while they compute).
-                const size_t dyn = park_bytes + io_bytes + (size_t)quad_model_f4(2) * sizeof(float4) + (s->zero_copy.on ? s->hostio_pad : 0);
-                TileArgs ta; ta.on = 1; ta.io_f4 = (int)(park_bytes / 16); ta.model_f4 = (int)((park_bytes + io_bytes) / 16);
-                ta.h_act = nullptr; ta.h_obs = ta.h_rew = nullptr; ta.h_reset = nullptr; ta.h_timeout = nullptr;
-                if (s->zero_copy.on) { ta.h_act = actions; ta.h_obs = s->zero_copy.obs; ta.h_rew = s->zero_copy.rew; ta.h_reset = s->zero_copy.reset; ta.h_timeout = s->zero_copy.timeout; }
-                const int qgrid = (int)N / epb;
-#define COMMA ,
-#define QLOCO(SP_, BK, HIO)                                                                                               \
-    do {                                                                                                                   \
-        int rc_ = set_smem(s, quad_loco_kernel<2, SP_, BK, HIO>, dyn); if (rc_) return rc_;                                \
-        cudaLaunchConfig_t lc = {};                                                                                        \
-        lc.gridDim = dim3(qgrid); lc.blockDim = dim3(BK); lc.dynamicSmemBytes = dyn; lc.stream = st;                       \
-        cudaLaunchAttribute at[1];                                                                                         \
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                     \
-        at[0].val.programmaticStreamSerializationAllowed = 1;                                                              \
-        lc.attrs = at; lc.numAttrs = 1;                                                                                    \
-        CUDA_TRY(cudaLaunchKernelEx(&lc, quad_loco_kernel<2, SP_, BK, HIO>, (const float4 *)s->d_qm, s->buf, P, actions, (int)N, (int)s->hm.substeps, ta)); \
-    } while (0)
-#define QLOCO_S(BK, HIO) do { if (s->quad_spec == 3) QLOCO(3, BK, HIO); else QLOCO(0, BK, HIO); } while (0)
-                // the plain task (no per-env physical parameters, no dof-force / net-contact tensors acquired): the lean instantiation
-                const bool lean = !s->buf.p[B2G_T_ENV_MASS_SCALE] && !s->buf.p[B2G_T_ENV_DOF_PROPS] && !s->buf.p[B2G_T_ENV_FRICTION] &&
-                                  !s->buf.p[B2G_T_NET_CONTACT] && !s->buf.p[B2G_T_DOF_FORCE] && !getenv_once("B2G_NO_LEAN");
-                if (qb == 128) { if (s->zero_copy.on) QLOCO_S(128, true); else QLOCO_S(128, false); }
-                else if (qb == 32) { if (s->zero_copy.on) QLOCO_S(32, true); else QLOCO_S(32, false); }
-                else if (s->zero_copy.on) QLOCO_S(64, true);
-                else if (lean) { if (s->quad_spec == 3) QLOCO(3, 64, false COMMA true); else QLOCO(0, 64, false COMMA true); }
-                else QLOCO_S(64, false);
-#undef QLOCO_S
-#undef QLOCO
-#undef COMMA
-                s->launches++;
-                CUDA_TRY(cudaGetLastError());
-                return B2G_OK;
-            }
-        }
-        // tiles by bulk copy: whole blocks only, every tile a multiple of 16 bytes at a 16-byte-aligned address
-        const int epb = blk / s->lanes, ndof = s->hm.nl - 1, O = P.num_obs, ns6 = 6 * s->hm.nsens;
-        const bool clip_sep = s->buf.p[B2G_T_OBS_CLIPPED] && s->buf.p[B2G_T_OBS_CLIPPED] != s->buf.p[B2G_T_OBS];
-        const size_t state_bytes = s->dyn_smem;                                   // slot state + accumulators
-        const size_t io_bytes = ((size_t)epb * (13 + 3 * ndof + ns6 + (hum ? ndof : 0)) * 4 + 15) & ~(size_t)15;
-        const size_t out_bytes = (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1);
-        const bool tiles = (N % epb == 0) && (epb % 16 == 0) && ((epb * ndof * 4) % 16 == 0) && ((epb * ns6 * 4) % 16 == 0) &&
-                           ((epb * O * 4) % 16 == 0) && out_bytes <= state_bytes && s->buf.p[B2G_T_ACTIONS];
-        const size_t model_bytes = offsetof(DevModel, slots) + (size_t)s->hm.ns * MAX_LANES * sizeof(SlotRec) + (((size_t)s->hm.nl * sizeof(LinkC) + 15) & ~(size_t)15) +
-                                   (((size_t)s->hm.ncp * sizeof(CpC) + 15) & ~(size_t)15);
-        const size_t io_used = tiles ? io_bytes : 16;
-        const size_t dyn = state_bytes + io_used + model_bytes;
-        TileArgs ta; ta.on = tiles ? 1 : 0; ta.io_f4 = (int)(state_bytes / 16); ta.model_f4 = (int)((state_bytes + io_used) / 16);
-        ta.h_act = nullptr; ta.h_obs = ta.h_rew = nullptr; ta.h_reset = nullptr; ta.h_timeout = nullptr;
-        if (s->zero_copy.on) {
-            if (!tiles) return fail(B2G_E_UNSUPPORTED, "zero-copy host step needs the tiled kernel");
-            ta.h_act = actions; ta.h_obs = s->zero_copy.obs; ta.h_rew = s->zero_copy.rew; ta.h_reset = s->zero_copy.reset; ta.h_timeout = s->zero_copy.timeout;
-        }
-#define LOCO_T(LN, HM, BK, TL) do { if (TL && s->zero_copy.on) LOCO_K(LN, HM, BK, TL, TL); else LOCO_K(LN, HM, BK, TL, false); } while (0)
-#define LOCO_K(LN, HM, BK, TL, HIO)                                                                                       \
-    do {                                                                                                                   \
-        int rc_ = set_smem(s, loco_step_kernel<LN, false, HM, BK, TL, HIO>, dyn); if (rc_) return rc_;                       \
-        cudaLaunchConfig_t lc = {};                                                                                        \
-        lc.gridDim = dim3(grid); lc.blockDim = dim3(blk); lc.dynamicSmemBytes = dyn; lc.stream = st;                       \
-        cudaLaunchAttribute at[1];                                                                                         \
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                     \
-        at[0].val.programmaticStreamSerializationAllowed = 1;                                                              \
-        lc.attrs = at; lc.numAttrs = 1;                                                                                    \
-        CUDA_TRY(cudaLaunchKernelEx(&lc, loco_step_kernel<LN, false, HM, BK, TL, HIO>, (const DevModel *)s->dm,            \
-                                    (const int16_t *)s->d_hf, s->buf, P, actions, (int)N, ta));                            \
-    } while (0)
-#define LOCO(LN, HM, BK) do { if (tiles) LOCO_T(LN, HM, BK, true); else LOCO_T(LN, HM, BK, false); } while (0)
-        if (s->d_hf) return fail(B2G_E_UNSUPPORTED, "locomotion tasks run on the ground plane");
-        if (s->hm.self_on) {             // link-link contact: separate instantiations (Humanoid-type tasks, device or staged I/O)
-#define LOCO_S(BK, TL)                                                                                                     \
-    do {                                                                                                                   \
-        int rc_ = set_smem(s, loco_step_kernel<4, false, true, BK, TL, false, true>, dyn); if (rc_) return rc_;            \
-        cudaLaunchConfig_t lc = {};                                                                                        \
-        lc.gridDim = dim3(grid); lc.blockDim = dim3(blk); lc.dynamicSmemBytes = dyn; lc.stream = st;                       \
-        cudaLaunchAttribute at[1];                                                                                         \
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                     \
-        at[0].val.programmaticStreamSerializationAllowed = 1;                                                              \
-        lc.attrs = at; lc.numAttrs = 1;                                                                                    \
-        CUDA_TRY(cudaLaunchKernelEx(&lc, loco_step_kernel<4, false, true, BK, TL, false, true>, (const DevModel *)s->dm,   \
-                                    (const int16_t *)s->d_hf, s->buf, P, actions, (int)N, ta));                            \
-    } while (0)
-            if (!hum || s->lanes != 4 || s->zero_copy.on) return fail(B2G_E_UNSUPPORTED, "self-collision: fused step instantiated for 4-lane Humanoid-type tasks with device or staged I/O");
-            if (blk == 64) { if (tiles) LOCO_S(64, true); else LOCO_S(64, false); }
-            else if (blk == 32) { if (tiles) LOCO_S(32, true); else LOCO_S(32, false); }
-            else return fail(B2G_E_UNSUPPORTED, "self-collision: no fused step instantiated for this CTA size");
-#undef LOCO_S
-        }
-        else if (!hum && s->lanes == 4 && blk == 128) LOCO(4, false, 128);
-        else if (!hum && s->lanes == 4 && blk == 64) LOCO(4, false, 64);
-        else if (!hum && s->lanes == 1 && blk == 128) LOCO(1, false, 128);
-        else if (hum && s->lanes == 4 && blk == 128) LOCO(4, true, 128);
-        else if (hum && s->lanes == 4 && blk == 64) LOCO(4, true, 64);
-        else if (hum && s->lanes == 4 && blk == 32) LOCO(4, true, 32);
-        else if (hum && s->lanes == 2 && blk == 64) LOCO(2, true, 64);
-        else if (hum && s->lanes == 2 && blk == 32) LOCO(2, true, 32);
-        else if (hum && s->lanes == 1 && blk == 64) LOCO(1, true, 64);
-        else if (hum && s->lanes == 1 && blk == 32) LOCO(1, true, 32);
-        else return fail(B2G_E_UNSUPPORTED, "no locomotion kernel instantiated for this (lanes, CTA size) combination");
-#undef LOCO
-#undef LOCO_T
-#undef LOCO_K
+        return launch(s, cartpole_step_kernel<128>, grid, blk, s->dyn_smem, st, SMEM, s->dm, s->buf, P, actions, (int)N);
     }
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    rc = require(s, {B2G_T_POTENTIALS, B2G_T_PREV_POTENTIALS, B2G_T_INITIAL_ROOT}, "b2g_task_step"); if (rc) return rc;
+    const bool hum = P.task == B2G_TASK_HUMANOID;
+    const int O = P.num_obs, ns6 = 6 * s->hm.nsens;
+    const bool clip_sep = s->buf.p[B2G_T_OBS_CLIPPED] && s->buf.p[B2G_T_OBS_CLIPPED] != s->buf.p[B2G_T_OBS];
+    // the output tiles, staged in the shared memory of the slot state: obs | obs_clipped? | rew | pot | ppot | up | head | reset | progress | timeout
+    auto out_bytes = [&](int epb) { return (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1); };
+    if (!hum && s->quad_ns == 2 && !s->d_hf) {           // Ant on the quad sub-step (whole tiles only)
+        constexpr int EPB = QUAD_LOCO_BLOCK / 4, ND = 8;
+        const size_t park_bytes = (size_t)quad_park_f4(2) * QUAD_LOCO_BLOCK * sizeof(float4);
+        const size_t io_bytes = ((size_t)EPB * (13 + 3 * ND + ns6) * 4 + 15) & ~(size_t)15;
+        if (whole_tiles(N, EPB) && out_bytes(EPB) <= park_bytes) {
+            const size_t dyn = park_bytes + io_bytes + (size_t)quad_model_f4(2) * sizeof(float4);
+            const bool lean = !s->buf.p[B2G_T_ENV_MASS_SCALE] && !s->buf.p[B2G_T_ENV_DOF_PROPS] && !s->buf.p[B2G_T_ENV_FRICTION] &&
+                              !s->buf.p[B2G_T_NET_CONTACT] && !s->buf.p[B2G_T_DOF_FORCE];
+            return launch(s, quad_loco_kernel_for(s->quad_spec, io != nullptr, lean), (int)N / EPB, QUAD_LOCO_BLOCK, dyn, st, SMEM_PDL,
+                          (const float4 *)s->d_qm, s->buf, P, actions, (int)N, (int)s->hm.substeps,
+                          tile_args(true, park_bytes, park_bytes + io_bytes, actions, io));
+        }
+    }
+    if (s->d_hf) return fail(B2G_E_UNSUPPORTED, "locomotion tasks run on the ground plane");
+    // tiles by bulk copy: whole blocks only, every tile a multiple of 16 bytes at a 16-byte-aligned address
+    const int epb = blk / s->lanes, ndof = s->hm.nl - 1;
+    const size_t state_bytes = s->dyn_smem;                                   // slot state + accumulators
+    const size_t io_bytes = ((size_t)epb * (13 + 3 * ndof + ns6 + (hum ? ndof : 0)) * 4 + 15) & ~(size_t)15;
+    const bool tiles = whole_tiles(N, epb) && out_bytes(epb) <= state_bytes && s->buf.p[B2G_T_ACTIONS];
+    const size_t model_bytes = offsetof(DevModel, slots) + (size_t)s->hm.ns * MAX_LANES * sizeof(SlotRec) + (((size_t)s->hm.nl * sizeof(LinkC) + 15) & ~(size_t)15) +
+                               (((size_t)s->hm.ncp * sizeof(CpC) + 15) & ~(size_t)15);
+    const size_t io_used = tiles ? io_bytes : 16;
+    const size_t dyn = state_bytes + io_used + model_bytes;
+    const LocoKernel k = loco_kernel_for(s->lanes, blk, hum, tiles, io != nullptr, s->hm.self_on);
+    if (!k) return fail(B2G_E_UNSUPPORTED, "no locomotion step kernel instantiated for this (lanes, CTA size, task, tiles, host I/O, self-collision) combination");
+    return launch(s, k, grid, blk, dyn, st, SMEM_PDL, (const DevModel *)s->dm, (const int16_t *)s->d_hf, s->buf, P, actions, (int)N,
+                  tile_args(tiles, state_bytes, state_bytes + io_used, actions, io));
 }
+
+// the fused Ant step on the quad sub-step: (specialisation, host I/O, lean); 64 threads, 16 envs per CTA.  Lean: the plain
+// task (no per-env physical parameters, no dof-force / net-contact tensors acquired), device or staged I/O
+static QuadLocoKernel quad_loco_kernel_for(int spec, bool hostio, bool lean) {
+    constexpr int B = QUAD_LOCO_BLOCK;
+    const bool sp3 = spec == 3;
+    if (hostio) return sp3 ? quad_loco_kernel<2, 3, B, true> : quad_loco_kernel<2, 0, B, true>;
+    if (lean) return sp3 ? quad_loco_kernel<2, 3, B, false, true> : quad_loco_kernel<2, 0, B, false, true>;
+    return sp3 ? quad_loco_kernel<2, 3, B, false> : quad_loco_kernel<2, 0, B, false>;
+}
+
+// the fused Ant / Humanoid step on the generic Stepper (ground plane): (lanes, CTA size, Humanoid, tiles, host I/O,
+// self-collision).  Host I/O needs the tiles; self-collision runs 4-lane Humanoid-type tasks with device or staged I/O.
+static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self) {
+    if (hostio && !tiles) return nullptr;
+    if (self) {
+        if (!hum || lanes != 4 || hostio) return nullptr;
+        if (block == 64) return tiles ? loco_step_kernel<4, false, true, 64, true, false, true> : loco_step_kernel<4, false, true, 64, false, false, true>;
+        if (block == 32) return tiles ? loco_step_kernel<4, false, true, 32, true, false, true> : loco_step_kernel<4, false, true, 32, false, false, true>;
+        return nullptr;
+    }
+#define LOCO_IO(L, HUM, B) (tiles ? (hostio ? loco_step_kernel<L, false, HUM, B, true, true> : loco_step_kernel<L, false, HUM, B, true, false>) \
+                                  : loco_step_kernel<L, false, HUM, B, false, false>)
+    if (!hum) {
+        switch (key(lanes, block)) {
+            case key(4, 128): return LOCO_IO(4, false, 128);
+            case key(4, 64): return LOCO_IO(4, false, 64);
+            case key(1, 128): return LOCO_IO(1, false, 128);
+        }
+        return nullptr;
+    }
+    switch (key(lanes, block)) {
+        case key(4, 128): return LOCO_IO(4, true, 128);
+        case key(4, 64): return LOCO_IO(4, true, 64);
+        case key(4, 32): return LOCO_IO(4, true, 32);
+        case key(2, 64): return LOCO_IO(2, true, 64);
+        case key(2, 32): return LOCO_IO(2, true, 32);
+        case key(1, 64): return LOCO_IO(1, true, 64);
+        case key(1, 32): return LOCO_IO(1, true, 32);
+    }
+#undef LOCO_IO
+    return nullptr;
+}
+
+extern "C" int b2g_task_step(b2g_sim *s, const float *actions, void *stream) { return task_step(s, actions, stream, nullptr); }
 
 // K x VecTask.step() with the actions of all K steps given up front (open-loop / random-action rollouts)
 extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, float *obs_out, float *rew_out, int64_t *reset_out,
@@ -1464,13 +1171,13 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     if (!s || !actions || !obs_out || !rew_out || !reset_out || K < 1) return fail(B2G_E_INVALID, "b2g_task_rollout: null argument or K < 1");
     if (!s->has_task && !s->has_anymal && !s->has_hand) return fail(B2G_E_INVALID, "b2g_task_rollout: call b2g_set_task first");
     const size_t N = s->num_envs;
-    const bool fused = s->has_task && s->task.task == B2G_TASK_ANT && s->quad_ns == 2 && !s->d_hf && (N % 16 == 0) &&
-                       ((16 * 6 * s->hm.nsens * 4) % 16 == 0);
+    constexpr int QB = 64, EPB = 16;
+    const bool fused = s->has_task && s->task.task == B2G_TASK_ANT && s->quad_ns == 2 && !s->d_hf && whole_tiles(N, EPB);
     cudaStream_t st = (cudaStream_t)stream;
     if (!fused) {
         // every other task / shape: K single steps, their results copied into the (K, N, .) outputs (same semantics, no fusion)
-        const int A = s->has_anymal ? s->anymal.num_actions : (s->has_hand ? s->hand.num_actions : s->task.num_actions);
-        const int O = s->has_anymal ? s->anymal.num_obs : (s->has_hand ? s->hand.num_obs : s->task.num_obs);
+        int A, O;
+        task_sizes(s, &A, &O);
         const void *obs_src = s->buf.p[B2G_T_OBS_CLIPPED] ? s->buf.p[B2G_T_OBS_CLIPPED] : s->buf.p[B2G_T_OBS];
         for (int k = 0; k < K; k++) {
             int rc = b2g_task_step(s, actions + (size_t)k * N * A, stream); if (rc) return rc;
@@ -1486,7 +1193,6 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     const b2g_task_params &P = s->task;
     if (s->buf_bytes[B2G_T_OBS] < N * P.num_obs * 4) return fail(B2G_E_INVALID, "OBS buffer too small");
     CUDA_TRY(cudaSetDevice(s->device));
-    constexpr int QB = 64, EPB = 16;
     const int nd_ = 8, O = P.num_obs, ns6 = 6 * s->hm.nsens;
     const size_t park_f4 = (size_t)quad_park_f4(2) * QB;
     const size_t io_f4 = ((size_t)EPB * (13 + 2 * nd_ + 2 * nd_ + ns6) * 4 + 15) / 16;
@@ -1497,23 +1203,8 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     ra.actions = actions; ra.obs_out = obs_out; ra.rew_out = rew_out; ra.reset_out = (long long *)reset_out; ra.timeout_out = timeout_out;
     ra.K = K; ra.io_f4 = (int)park_f4; ra.model_f4 = (int)(park_f4 + io_f4); ra.stage_f4 = (int)(park_f4 + io_f4 + model_f4);
     const size_t dyn = (park_f4 + io_f4 + model_f4 + stage_f4) * 16;
-    const int grid = (int)N / EPB;
-#define QROLL(SP_)                                                                                                         \
-    do {                                                                                                                   \
-        int rc_ = set_smem(s, quad_rollout_kernel<2, SP_>, dyn); if (rc_) return rc_;                                      \
-        cudaLaunchConfig_t lc = {};                                                                                        \
-        lc.gridDim = dim3(grid); lc.blockDim = dim3(QB); lc.dynamicSmemBytes = dyn; lc.stream = st;                        \
-        cudaLaunchAttribute at[1];                                                                                         \
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                     \
-        at[0].val.programmaticStreamSerializationAllowed = 1;                                                              \
-        lc.attrs = at; lc.numAttrs = 1;                                                                                    \
-        CUDA_TRY(cudaLaunchKernelEx(&lc, quad_rollout_kernel<2, SP_>, (const float4 *)s->d_qm, s->buf, P, (int)N, (int)s->hm.substeps, ra)); \
-    } while (0)
-    if (s->quad_spec == 3) QROLL(3); else QROLL(0);
-#undef QROLL
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    return launch(s, s->quad_spec == 3 ? quad_rollout_kernel<2, 3> : quad_rollout_kernel<2, 0>, (int)N / EPB, QB, dyn, st, SMEM_PDL,
+                  (const float4 *)s->d_qm, s->buf, P, (int)N, (int)s->hm.substeps, ra);
 }
 
 // VecTask.reset_done() (vec_task.py:440-455): reset_idx of every env whose reset_buf is set, right now (stream-ordered)
@@ -1528,18 +1219,15 @@ extern "C" int b2g_reset_flagged(b2g_sim *s, void *stream) {
         rc = require(s, {B2G_T_COMMANDS, B2G_T_FEET_AIR_TIME, B2G_T_EPISODE_SUMS, B2G_T_REDUCE_SCRATCH}, "b2g_reset_flagged(AnymalTerrain)"); if (rc) return rc;
         if (s->anymal.custom_origins) { rc = require(s, {B2G_T_ENV_ORIGINS, B2G_T_TERRAIN_LEVELS, B2G_T_TERRAIN_TYPES, B2G_T_TERRAIN_ORIGINS}, "b2g_reset_flagged(AnymalTerrain)"); if (rc) return rc; }
         CUDA_TRY(cudaMemsetAsync((float *)s->buf.p[B2G_T_REDUCE_SCRATCH] + REDUCE_PARTIALS, 0, 16 * sizeof(float), st));
-        anymal_reset_obs_kernel<32, 128><<<(N * 32 + 127) / 128, 128, 0, st>>>(s->buf, s->anymal, s->d_hf, N, nd, 0, s->step_counter, 1);
-    } else if (s->has_hand) {
+        return launch(s, anymal_reset_obs_kernel<32, 128>, (N * 32 + 127) / 128, 128, 0, st, PLAIN, s->buf, s->anymal, s->d_hf, N, nd, 0, s->step_counter, 1);
+    }
+    if (s->has_hand) {
         rc = require(s, {B2G_T_INITIAL_ROOT, B2G_T_GOAL_STATES, B2G_T_DOF_TARGET, B2G_T_PREV_TARGETS, B2G_T_SUCCESSES, B2G_T_RESET_GOAL}, "b2g_reset_flagged(ShadowHand)"); if (rc) return rc;
         if (s->hand.force_scale > 0.f) { rc = require(s, {B2G_T_OBJ_FORCE, B2G_T_RANDOM_FORCE_PROB}, "b2g_reset_flagged(ShadowHand, forceScale > 0)"); if (rc) return rc; }
-        hand_reset_kernel<<<(N + 127) / 128, 128, 0, st>>>(s->buf, s->hand, N, nd);
-    } else {
-        if (s->task.task != B2G_TASK_CARTPOLE) { rc = require(s, {B2G_T_POTENTIALS, B2G_T_PREV_POTENTIALS, B2G_T_INITIAL_ROOT}, "b2g_reset_flagged"); if (rc) return rc; }
-        loco_reset_kernel<<<(N + 127) / 128, 128, 0, st>>>(s->buf, s->task, N, nd);
+        return launch(s, hand_reset_kernel, (N + 127) / 128, 128, 0, st, PLAIN, s->buf, s->hand, N, nd);
     }
-    s->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return B2G_OK;
+    if (s->task.task != B2G_TASK_CARTPOLE) { rc = require(s, {B2G_T_POTENTIALS, B2G_T_PREV_POTENTIALS, B2G_T_INITIAL_ROOT}, "b2g_reset_flagged"); if (rc) return rc; }
+    return launch(s, loco_reset_kernel, (N + 127) / 128, 128, 0, st, PLAIN, s->buf, s->task, N, nd);
 }
 
 extern "C" int b2g_task_step_host(b2g_sim *s, const float *h_actions, float *h_obs, float *h_rew, int64_t *h_reset,
@@ -1548,32 +1236,30 @@ extern "C" int b2g_task_step_host(b2g_sim *s, const float *h_actions, float *h_o
     if (!s->has_task && !s->has_anymal && !s->has_hand) return fail(B2G_E_INVALID, "b2g_task_step_host: call b2g_set_task first");
     CUDA_TRY(cudaSetDevice(s->device));
     cudaStream_t st = (cudaStream_t)stream;
-    const int n_act = s->has_anymal ? s->anymal.num_actions : (s->has_hand ? s->hand.num_actions : s->task.num_actions);
-    const int n_obs = s->has_anymal ? s->anymal.num_obs : (s->has_hand ? s->hand.num_obs : s->task.num_obs);
+    int n_act, n_obs;
+    task_sizes(s, &n_act, &n_obs);
     const size_t N = s->num_envs, abytes = N * n_act * 4;
-    // fast path (Ant / Humanoid tiled kernel, every host buffer pinned): no copy launches at all
-    if (s->has_task && s->task.task != B2G_TASK_CARTPOLE && !s->no_zero_copy) {
+    // fast path (Ant / Humanoid tiled kernel, every host buffer pinned): no copy launches at all.  This pre-check counts the
+    // generic step's envs per CTA even when Ant runs the quad kernel (16 per CTA), so some env counts the quad kernel could
+    // tile take the staged path; a step that turns out untiled returns B2G_E_UNSUPPORTED and takes it as well.
+    if (s->has_task && s->task.task != B2G_TASK_CARTPOLE) {
         auto pinned = [](const void *p) {
             if (!p) return true;
             cudaPointerAttributes a;
             if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
             return a.type == cudaMemoryTypeHost;
         };
-        const int epb = s->block / s->lanes, ndof = s->hm.nl - 1;
-        const bool tiles_ok = (N % epb == 0) && (epb % 16 == 0) && ((epb * ndof * 4) % 16 == 0) && ((epb * 6 * s->hm.nsens * 4) % 16 == 0) &&
-                              ((epb * n_obs * 4) % 16 == 0) && s->buf.p[B2G_T_ACTIONS] && !s->d_hf;
-        if (tiles_ok && pinned(h_actions) && pinned(h_obs) && pinned(h_rew) && pinned(h_reset) && pinned(h_timeout)) {
-            s->zero_copy.on = true; s->zero_copy.obs = h_obs; s->zero_copy.rew = h_rew;
-            s->zero_copy.reset = (long long *)h_reset; s->zero_copy.timeout = h_timeout;
-            int rc = b2g_task_step(s, h_actions, stream);
-            s->zero_copy.on = false;
+        if (whole_tiles(N, s->block / s->lanes) && s->buf.p[B2G_T_ACTIONS] && !s->d_hf &&
+            pinned(h_actions) && pinned(h_obs) && pinned(h_rew) && pinned(h_reset) && pinned(h_timeout)) {
+            const HostOut io = {h_obs, h_rew, (long long *)h_reset, h_timeout};
+            const int rc = task_step(s, h_actions, stream, &io);
             if (rc == B2G_OK) { CUDA_TRY(cudaStreamSynchronize(st)); return B2G_OK; }
-            if (rc != B2G_E_UNSUPPORTED) return rc;       // else: the generic path below
+            if (rc != B2G_E_UNSUPPORTED) return rc;       // else: the staged path below
         }
     }
     if (!s->d_actions_stage) CUDA_TRY(cudaMalloc(&s->d_actions_stage, abytes));
     CUDA_TRY(cudaMemcpyAsync(s->d_actions_stage, h_actions, abytes, cudaMemcpyHostToDevice, st));
-    int rc = b2g_task_step(s, s->d_actions_stage, stream); if (rc) return rc;
+    int rc = task_step(s, s->d_actions_stage, stream, nullptr); if (rc) return rc;
     const void *obs_src = s->buf.p[B2G_T_OBS_CLIPPED] ? s->buf.p[B2G_T_OBS_CLIPPED] : s->buf.p[B2G_T_OBS];
     if (h_obs) CUDA_TRY(cudaMemcpyAsync(h_obs, obs_src, N * n_obs * 4, cudaMemcpyDeviceToHost, st));
     if (h_rew) CUDA_TRY(cudaMemcpyAsync(h_rew, s->buf.p[B2G_T_REW], N * 4, cudaMemcpyDeviceToHost, st));

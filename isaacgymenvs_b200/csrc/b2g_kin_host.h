@@ -8,6 +8,17 @@
 
 namespace b2g {
 
+// Unit quaternion (x, y, z, w) -> row-major rotation matrix, for the model constants built on the host (here, b2g_quad_host.h,
+// b2g_model_host.h).  Not the device quat_to_mat: that one scales by b2g_rsqrt, which moves the constants in the last bit.
+static inline void host_quat_to_mat(const float *q, float R[9]) {
+    float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
+    x /= n; y /= n; z /= n; w /= n;
+    const float M[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                        2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                        2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+    memcpy(R, M, sizeof(M));
+}
+
 // returns 0, or -1 when the articulation exceeds the kernel's limits (one lane per link and per body)
 static inline int kin_build(const b2g_model *m, int root_stride, KinModel &k) {
     memset(&k, 0, sizeof(k));
@@ -26,13 +37,7 @@ static inline int kin_build(const b2g_model *m, int root_stride, KinModel &k) {
         if (k.depth[i] > k.maxdepth) k.maxdepth = k.depth[i];
         k.slide[i] = (i && m->jtype[i] == 1) ? 1 : 0;
         if (i) { if (k.nchild[p] == KIN_MAX_CHILD) return -1; k.child[p][k.nchild[p]++] = i; }
-        const float *q = m->lquat + 4 * i;
-        float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
-        x /= n; y /= n; z /= n; w /= n;
-        const float R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                            2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                            2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-        memcpy(k.R0[i], R, sizeof(R));
+        host_quat_to_mat(m->lquat + 4 * i, k.R0[i]);
         for (int c = 0; c < 3; c++) { k.lpos[i][c] = m->lpos[3 * i + c]; k.axis[i][c] = m->axis[3 * i + c]; k.com[i][c] = m->com[3 * i + c]; }
         for (int c = 0; c < 6; c++) k.Ic[i][c] = m->inertia[6 * i + c];
         k.mass[i] = m->mass[i]; k.armature[i] = m->armature[i];

@@ -1,12 +1,13 @@
 // b2g_quad_host.h -- host side of the quad path (b2g_quad.cuh): decides whether an articulation is "four equal
 // hinge chains on a free base" and packs its constants into the quad model blob.  Plain C++ (no CUDA), shared by
-// b200gym.cu (b2g_create) and tests/quad_host.cu (the CPU run of the same arithmetic against the oracle).
+// b2g_model_host.h (b2g_create) and tests/quad_host.cu (the CPU run of the same arithmetic against the oracle).
 #pragma once
 #include <math.h>
 #include <string.h>
 #include <vector>
 #include "../../include/b200gym.h"
 #include "b2g_quad.cuh"
+#include "b2g_kin_host.h"
 
 namespace b2g {
 
@@ -129,12 +130,8 @@ static inline int quad_build(const b2g_model *m, const b2g_sim_params *sp, std::
         const int li = leg_link[l * NS + s];
         float L[QL_F4 * 4];
         memset(L, 0, sizeof(L));
-        const float *q = m->lquat + 4 * li;
-        float x = q[0], y = q[1], z = q[2], w = q[3], n = sqrtf(x * x + y * y + z * z + w * w);
-        x /= n; y /= n; z /= n; w /= n;
-        const float R0[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                             2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                             2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+        float R0[9];
+        host_quat_to_mat(m->lquat + 4 * li, R0);
         float a[3] = {m->axis[3 * li], m->axis[3 * li + 1], m->axis[3 * li + 2]};
         const float an = sqrtf(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
         if (!(an > 0.f)) return 0;
