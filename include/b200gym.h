@@ -176,7 +176,10 @@ enum {
      * kernels and the generic one). */
     B2G_T_ENV_MASS_SCALE = 42, /* f32 (N,L)   factor on every link's mass AND rotational inertia (rigid_body_properties.mass is set with
                                   recomputeInertia = True: utils/dr_utils.py:62); the COM stays */
-    B2G_T_ENV_DOF_PROPS = 43,  /* f32 (N,D,4) damping, stiffness, lower, upper of every DOF (dof_properties) */
+    B2G_T_ENV_DOF_PROPS = 43,  /* f32 (N,D,4) damping, stiffness, lower, upper of every DOF (dof_properties).  For a position-driven DOF
+                                  the columns are what get_actor_dof_properties reports for it: damping is all of its velocity
+                                  damping (the model's joint damping plus the drive's kd, applied as joint damping), stiffness the
+                                  drive's kp; the model's passive stiffness of that DOF stays */
     /* gym.acquire_jacobian_tensor / acquire_mass_matrix_tensor (tasks/franka_cube_stack.py:388-392); shapes from b2g_kin_shape:
      * nc = D for a fixed base, 6 + D for a floating base (base columns first: world linear, world angular velocity of the
      * root origin); rows = B - 1 for a fixed base (no row for the base body), B otherwise */
@@ -188,7 +191,19 @@ enum {
      * reset); b2g_simulate only reads OBJ_FORCE.  NULL = no force. */
     B2G_T_OBJ_FORCE = 46,      /* f32 (N,3) */
     B2G_T_RANDOM_FORCE_PROB = 47, /* f32 (N)   random_force_prob, shadow_hand.py:198,642 */
-    B2G_T_COUNT = 48
+    /* physical domain randomisation of a sim with a free object (ShadowHand's actor_params.object, tendon_properties and
+     * sim_params.gravity, vec_task.py:722-828).  NULL = the model's own values; b2g_bind refuses them (B2G_E_UNSUPPORTED) on a
+     * sim without a free object.  Any per-env parameter bound on such a sim (these three or ENV_MASS_SCALE / ENV_DOF_PROPS /
+     * ENV_FRICTION) selects the randomised instantiation of its simulate and ShadowHand step kernels.  Frictions combine as
+     * PhysX's default, the average of the two materials: ENV_FRICTION (the articulation's shapes) with the ground and with the
+     * object, the object's with the ground; where only one of ENV_FRICTION / ENV_OBJ_PROPS is bound, obj_mu stands in for the
+     * other material. */
+    B2G_T_ENV_OBJ_PROPS = 48,  /* f32 (N,4)  the object's size scale s (contact extents obj_half and obj_round x s; mass unchanged,
+                                  inertia x s^2), mass factor (mass, inertia and the contact gains obj_kn / obj_cn, which are
+                                  proportional to the mass), friction, unused */
+    B2G_T_ENV_TENDON_DAMPING = 49, /* f32 (N,nten)  damping of each tendon (ten_d) */
+    B2G_T_GRAVITY = 50,        /* f32 (3)    the sim's gravity, read on the device by every sub-step (bodies with gravity on) */
+    B2G_T_COUNT = 51
 };
 
 /* fused per-task control steps */

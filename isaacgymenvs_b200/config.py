@@ -41,6 +41,31 @@ def _num_envs(root, default):
     return default if root["num_envs"] in ("", None) else int(root["num_envs"])
 
 
+# cfg/task/ShadowHand.yaml randomization_params (the same block as ShadowHandOpenAI_FF.yaml / ShadowHandTest.yaml): what
+# task.randomize=True turns on
+def _dr(lo, hi, op, dist, **kw):
+    return {"range": [lo, hi], "operation": op, "distribution": dist, **kw}
+
+
+_SHADOW_HAND_DR = {
+    "frequency": 720,
+    "observations": _dr(0, .002, "additive", "gaussian", range_correlated=[0, .001]),
+    "actions": _dr(0., .05, "additive", "gaussian", range_correlated=[0, .015]),
+    "sim_params": {"gravity": _dr(0, 0.4, "additive", "gaussian")},
+    "actor_params": {
+        "hand": {"color": True,
+                 "tendon_properties": {"damping": _dr(0.3, 3.0, "scaling", "loguniform"),
+                                       "stiffness": _dr(0.75, 1.5, "scaling", "loguniform")},
+                 "dof_properties": {"damping": _dr(0.3, 3.0, "scaling", "loguniform"),
+                                    "stiffness": _dr(0.75, 1.5, "scaling", "loguniform"),
+                                    "lower": _dr(0, 0.01, "additive", "gaussian"), "upper": _dr(0, 0.01, "additive", "gaussian")},
+                 "rigid_body_properties": {"mass": _dr(0.5, 1.5, "scaling", "uniform", setup_only=True)},
+                 "rigid_shape_properties": {"friction": _dr(0.7, 1.3, "scaling", "uniform", num_buckets=250)}},
+        "object": {"scale": _dr(0.95, 1.05, "scaling", "uniform", setup_only=True),
+                   "rigid_body_properties": {"mass": _dr(0.5, 1.5, "scaling", "uniform", setup_only=True)},
+                   "rigid_shape_properties": {"friction": _dr(0.7, 1.3, "scaling", "uniform", num_buckets=250)}}}}
+
+
 def _builtin_task(name, root):
     """Python restatement of cfg/task/{Cartpole,Ant,Humanoid}.yaml (values only)."""
     plane = {"staticFriction": 1.0, "dynamicFriction": 1.0, "restitution": 0.0}
@@ -94,7 +119,7 @@ def _builtin_task(name, root):
                                   "assetFileNamePen": "mjcf/open_ai_assets/hand/pen.xml"},
                         "enableCameraSensors": False},
                 "sim": sim,
-                "task": {"randomize": False, "randomization_params": {}}}
+                "task": {"randomize": False, "randomization_params": copy.deepcopy(_SHADOW_HAND_DR)}}
     if name == "AnymalTerrain":
         sim = _sim(root, _physx(root, num_velocity_iterations=1, max_depenetration_velocity=100.0, contact_collection=1))
         sim.update({"dt": 0.005, "substeps": 1})

@@ -75,9 +75,9 @@ __device__ __forceinline__ Tiles prologue(DevModel *sm, uint64_t *mbar, const De
 }
 
 
-template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false>
-__device__ __forceinline__ Stepper<L, HF, BLOCK, OBJ, SELF> make_stepper(const DevModel *sm, const int16_t *hf, int lane) {
-    Stepper<L, HF, BLOCK, OBJ, SELF> st;
+template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false, bool DR = false>
+__device__ __forceinline__ Stepper<L, HF, BLOCK, OBJ, SELF, DR> make_stepper(const DevModel *sm, const int16_t *hf, int lane) {
+    Stepper<L, HF, BLOCK, OBJ, SELF, DR> st;
     st.m = sm; st.gr = Ground{sm, hf, sm->cps, -1.f};
     st.slots = &sm->slots[0][0]; st.links = sm->links;
     if (OBJ) {      // [link][k][env] layout: the env's column
@@ -89,7 +89,7 @@ __device__ __forceinline__ Stepper<L, HF, BLOCK, OBJ, SELF> make_stepper(const D
     }
     st.lane = lane;
     st.gmodel = nullptr;
-    st.dr_mass = nullptr; st.dr_dof = nullptr;
+    st.dr_mass = nullptr; st.dr_dof = nullptr; st.dr_ten = nullptr; st.dr_grav = nullptr;
     st.scen = nullptr; st.scs = 1;
     if (SELF) {
         if (sm->self_f4) st.scen = b2g_dyn_smem + (sm->ns * SLOT_F4 + sm->nacc * ACC_F4) * BLOCK + (threadIdx.x / L) * sm->self_f4;
@@ -109,6 +109,22 @@ __device__ __forceinline__ void attach_env_params_generic(ST &st, const DevModel
     if (envmu) st.gr.env_mu = 0.5f * (envmu[e] + sm.ground_mu);      // PhysX default combine mode: the average of the two materials
 }
 
+// the free object's per-env parameters, the tendon damping and the gravity (the DR instantiations of the free-object kernels;
+// null = the model's own).  Frictions combine as PhysX does by default, the average of the two materials: hand (ENV_FRICTION)
+// with object (ENV_OBJ_PROPS.z) for their contacts, object with ground for the object's ground contacts.  Where only one of the
+// two tensors is bound, the model's object friction obj_mu stands in for the missing material.
+template <class ST>
+__device__ __forceinline__ void attach_object_params(ST &st, const DevModel &sm, const Buffers &B, int e) {
+    const float4 *op = (const float4 *)B.p[B2G_T_ENV_OBJ_PROPS];
+    const float *hand_mu = (const float *)B.p[B2G_T_ENV_FRICTION];
+    const float *td = (const float *)B.p[B2G_T_ENV_TENDON_DAMPING];
+    const float4 v = op ? op[e] : make_float4(1.f, 1.f, sm.obj_mu, 0.f);
+    const float mu_h = hand_mu ? hand_mu[e] : sm.obj_mu;
+    st.set_obj_params(v.x, v.y, (op || hand_mu) ? 0.5f * (mu_h + v.z) : sm.obj_mu, op ? 0.5f * (v.z + sm.ground_mu) : sm.obj_mu);
+    if (td) st.dr_ten = td + (size_t)e * sm.nten;
+    st.dr_grav = (const float *)B.p[B2G_T_GRAVITY];
+}
+
 template <class ST>
 __device__ __forceinline__ typename ST::Outputs make_outputs(const DevModel &sm, const Buffers &B, int e, bool valid) {
     typename ST::Outputs o;
@@ -123,21 +139,22 @@ __device__ __forceinline__ typename ST::Outputs make_outputs(const DevModel &sm,
 
 // -------------------------------------------------------------------------------------------
 // gym.simulate(): physics only
-template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false>
+template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false, bool DR = false>
 __global__ void __launch_bounds__(BLOCK) simulate_kernel(const DevModel *__restrict__ gm, const int16_t *__restrict__ hf,
                                                          Buffers B, int N) {
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
     prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
-    using ST = Stepper<L, HF, BLOCK, OBJ, SELF>;
+    using ST = Stepper<L, HF, BLOCK, OBJ, SELF, DR>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;
     const bool valid = env < N;
     const int e = valid ? env : N - 1;
     const int nd = sm.nl - 1, NS = sm.ns;
-    ST st = make_stepper<L, HF, BLOCK, OBJ, SELF>(&sm, hf, lane);
+    ST st = make_stepper<L, HF, BLOCK, OBJ, SELF, DR>(&sm, hf, lane);
     st.gmodel = gm;
     attach_env_params_generic(st, sm, B, e);
+    if (DR) attach_object_params(st, sm, B, e);
     float *const root_row = (float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e * sm.root_stride;
     RootState rs; load_root(root_row, rs);
     ObjState ob;
@@ -717,11 +734,16 @@ extern "C" int b2g_bind(b2g_sim *s, int32_t slot, void *ptr, size_t bytes) {
         case B2G_T_ENV_FRICTION: need = (size_t)N * 4; break;
         case B2G_T_OBJ_FORCE: need = (size_t)N * 12; break;
         case B2G_T_RANDOM_FORCE_PROB: need = (size_t)N * 4; break;
+        case B2G_T_ENV_OBJ_PROPS: need = (size_t)N * 16; break;
+        case B2G_T_ENV_TENDON_DAMPING: need = (size_t)N * s->hm.nten * 4; break;
+        case B2G_T_GRAVITY: need = 12; break;
         case B2G_T_JACOBIAN: need = (size_t)N * s->hk.rows * 6 * s->hk.nc * 4; break;
         case B2G_T_MASS_MATRIX: need = (size_t)N * s->hk.nc * s->hk.nc * 4; break;
         default: need = 0; break;   // ACTIONS / OBS / OBS_CLIPPED are checked against the task in b2g_set_task
     }
     if (ptr && bytes < need) return fail(B2G_E_INVALID, "b2g_bind: buffer smaller than the tensor's layout requires");
+    if ((slot == B2G_T_ENV_OBJ_PROPS || slot == B2G_T_ENV_TENDON_DAMPING || slot == B2G_T_GRAVITY) && !s->hm.obj_on)
+        return fail(B2G_E_UNSUPPORTED, "b2g_bind: object, tendon and gravity parameters need a sim with a free object");
     s->buf.p[slot] = ptr; s->buf_bytes[slot] = bytes;
     return B2G_OK;
 }
@@ -796,10 +818,11 @@ static QuadSimKernel quad_simulate_kernel_for(int ns, bool hf, int spec) {
     return nullptr;
 }
 
-// gym.simulate() on the generic Stepper: (lanes, CTA size, height field, free object, self-collision)
+// gym.simulate() on the generic Stepper: (lanes, CTA size, height field, free object, self-collision, per-env physical
+// parameters of the free-object sim bound)
 using SimulateKernel = void (*)(const DevModel *, const int16_t *, Buffers, int);
-static SimulateKernel simulate_kernel_for(int lanes, int block, bool hf, bool obj, bool self) {
-    if (obj) {                   // the free object (b2g_create_ext keeps it on the ground plane)
+static SimulateKernel simulate_kernel_for(int lanes, int block, bool hf, bool obj, bool self, bool dr) {
+    if (obj && !dr) {            // the free object (b2g_create_ext keeps it on the ground plane)
         switch (key(lanes, block)) {
             case key(8, 128): return simulate_kernel<8, false, 128, true>;
             case key(8, 64): return simulate_kernel<8, false, 64, true>;
@@ -821,19 +844,31 @@ static SimulateKernel simulate_kernel_for(int lanes, int block, bool hf, bool ob
         }
         return nullptr;
     }
-    if (hf && key(lanes, block) != key(4, 128)) return nullptr;          // the height field: 4 lanes, 128 threads
-    switch (key(lanes, block)) {
-        case key(4, 128): return !hf ? simulate_kernel<4, false, 128> : simulate_kernel<4, true, 128>;
-        case key(4, 64): return simulate_kernel<4, false, 64>;
-        case key(4, 32): return simulate_kernel<4, false, 32>;
-        case key(2, 128): return simulate_kernel<2, false, 128>;
-        case key(2, 64): return simulate_kernel<2, false, 64>;
-        case key(2, 32): return simulate_kernel<2, false, 32>;
-        case key(1, 128): return simulate_kernel<1, false, 128>;
-        case key(1, 64): return simulate_kernel<1, false, 64>;
-        case key(1, 32): return simulate_kernel<1, false, 32>;
+    if (!obj) {
+        if (hf && key(lanes, block) != key(4, 128)) return nullptr;      // the height field: 4 lanes, 128 threads
+        switch (key(lanes, block)) {
+            case key(4, 128): return !hf ? simulate_kernel<4, false, 128> : simulate_kernel<4, true, 128>;
+            case key(4, 64): return simulate_kernel<4, false, 64>;
+            case key(4, 32): return simulate_kernel<4, false, 32>;
+            case key(2, 128): return simulate_kernel<2, false, 128>;
+            case key(2, 64): return simulate_kernel<2, false, 64>;
+            case key(2, 32): return simulate_kernel<2, false, 32>;
+            case key(1, 128): return simulate_kernel<1, false, 128>;
+            case key(1, 64): return simulate_kernel<1, false, 64>;
+            case key(1, 32): return simulate_kernel<1, false, 32>;
+        }
+        return nullptr;
     }
-    return nullptr;
+    // the free object with per-env physical parameters: the hand's 4 lanes, 128 threads
+    return key(lanes, block) == key(4, 128) ? simulate_kernel<4, false, 128, true, false, true> : nullptr;
+}
+
+// a free-object sim with any per-env physical parameter bound runs the DR instantiation of its kernels
+static bool object_dr_bound(const b2g_sim *s) {
+    if (!s->hm.obj_on) return false;
+    for (int k : {B2G_T_ENV_MASS_SCALE, B2G_T_ENV_DOF_PROPS, B2G_T_ENV_FRICTION, B2G_T_ENV_OBJ_PROPS, B2G_T_ENV_TENDON_DAMPING, B2G_T_GRAVITY})
+        if (s->buf.p[k]) return true;
+    return false;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -850,8 +885,8 @@ extern "C" int b2g_simulate(b2g_sim *s, void *stream) {
                       QUAD_SIM_BLOCK, dyn, st, SMEM, s->d_qm, s->d_hf, s->buf, N, s->hm.substeps);
     }
     const int blk = s->block, grid = (N * s->lanes + blk - 1) / blk;
-    const SimulateKernel k = simulate_kernel_for(s->lanes, blk, s->d_hf != nullptr, s->hm.obj_on, s->hm.self_on);
-    if (!k) return fail(B2G_E_UNSUPPORTED, "no simulate kernel instantiated for this (lanes, CTA size, terrain, free object, self-collision) combination");
+    const SimulateKernel k = simulate_kernel_for(s->lanes, blk, s->d_hf != nullptr, s->hm.obj_on, s->hm.self_on, object_dr_bound(s));
+    if (!k) return fail(B2G_E_UNSUPPORTED, "no simulate kernel instantiated for this (lanes, CTA size, terrain, free object, self-collision, randomised) combination");
     return launch(s, k, grid, blk, s->dyn_smem, st, SMEM, s->dm, s->d_hf, s->buf, N);
 }
 
@@ -972,18 +1007,21 @@ extern "C" int b2g_set_hand_task(b2g_sim *s, const b2g_hand_params *t) {
     return B2G_OK;
 }
 
-// the fused ShadowHand step: (lanes, CTA size)
+// the fused ShadowHand step: (lanes, CTA size, per-env physical parameters bound)
 using HandKernel = void (*)(const DevModel *, Buffers, b2g_hand_params, HandDev, const float *, int);
-static HandKernel hand_kernel_for(int lanes, int block) {
-    switch (key(lanes, block)) {
-        case key(8, 128): return hand_step_kernel<8, 128>;
-        case key(8, 64): return hand_step_kernel<8, 64>;
-        case key(4, 128): return hand_step_kernel<4, 128>;
-        case key(4, 64): return hand_step_kernel<4, 64>;
-        case key(4, 32): return hand_step_kernel<4, 32>;
-        case key(1, 32): return hand_step_kernel<1, 32>;
+static HandKernel hand_kernel_for(int lanes, int block, bool dr) {
+    if (!dr) {
+        switch (key(lanes, block)) {
+            case key(8, 128): return hand_step_kernel<8, 128>;
+            case key(8, 64): return hand_step_kernel<8, 64>;
+            case key(4, 128): return hand_step_kernel<4, 128>;
+            case key(4, 64): return hand_step_kernel<4, 64>;
+            case key(4, 32): return hand_step_kernel<4, 32>;
+            case key(1, 32): return hand_step_kernel<1, 32>;
+        }
+        return nullptr;
     }
-    return nullptr;
+    return key(lanes, block) == key(4, 128) ? hand_step_kernel<4, 128, true> : nullptr;     // the hand's 4 lanes, 128 threads
 }
 
 static int hand_step(b2g_sim *s, const float *actions, void *stream) {
@@ -1002,8 +1040,8 @@ static int hand_step(b2g_sim *s, const float *actions, void *stream) {
     if (s->buf_bytes[B2G_T_OBS] < N * P.num_obs * 4) return fail(B2G_E_INVALID, "OBS buffer too small");
     CUDA_TRY(cudaSetDevice(s->device));
     const int blk = s->block, grid = ((int)N * s->lanes + blk - 1) / blk;
-    const HandKernel k = hand_kernel_for(s->lanes, blk);
-    if (!k) return fail(B2G_E_UNSUPPORTED, "no ShadowHand kernel instantiated for this (lanes, CTA size) combination");
+    const HandKernel k = hand_kernel_for(s->lanes, blk, object_dr_bound(s));
+    if (!k) return fail(B2G_E_UNSUPPORTED, "no ShadowHand kernel instantiated for this (lanes, CTA size, randomised) combination");
     return launch(s, k, grid, blk, s->dyn_smem, (cudaStream_t)stream, SMEM, s->dm, s->buf, P, s->hand_dev, actions, (int)N);
 }
 

@@ -543,8 +543,10 @@ struct ObjPose {              // the object at the start of the sub-step, as the
     float Ro[9], c[3], w[3], vO[3];
 };
 
-// SELF: link-link contact code compiled in (the kernels instantiate it separately: the default path carries none of it)
-template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false>
+// SELF: link-link contact code compiled in (the kernels instantiate it separately: the default path carries none of it).
+// DR (with OBJ): the per-env object, tendon and gravity parameters of physical domain randomisation are read (a separate
+// instantiation, chosen at run time when a randomisation tensor is bound: the default path carries none of it)
+template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false, bool DR = false>
 struct Stepper {
     const DevModel *m;        // header (scalars, sensor tables)
     const SlotRec *slots;     // [ns][MAX_LANES]
@@ -555,7 +557,10 @@ struct Stepper {
     int lane;
     const DevModel *gmodel;   // the model's copy in global memory (self-collision tables), may be null when self_on == 0
     const float *dr_mass;     // per-env physical parameters (vec_task.py:720-828 as arrays; null = the model's own): this env's link-mass
-    const float4 *dr_dof;     // factors [nl] (inertia scales with the mass), and per DOF (damping, stiffness, lower, upper)
+    const float4 *dr_dof;     // factors [nl] (inertia scales with the mass), and per DOF (damping, stiffness, lower, upper; kd, kp, lower,
+                              // upper of a position-driven DOF)
+    const float *dr_ten;      // DR: this env's damping of each tendon [nten] (null = the model's ten_d)
+    const float *dr_grav;     // DR: the sim's gravity (3), global memory (null = the model's)
     float4 *scen;             // this ENV's self-collision scratch, element i at scen[i * scs]: [0, ncp) sphere centres about O +
     int scs;                  // radius, [ncp].x hit count, [ncp + 1, ncp + 5) the overlapping pairs of this sub-step (SELF_HITS x uint16)
 
@@ -782,9 +787,10 @@ struct Stepper {
                 const float4 a = S4x(r0 >> 8, r0 & 255, 6), b = S4x(r1 >> 8, r1 & 255, 6);
                 const float c0 = m->ten_coef[t][0], c1 = m->ten_coef[t][1];
                 const float len = c0 * a.z + c1 * b.z, rate = c0 * a.w + c1 * b.w;
+                const float td = (DR && dr_ten) ? dr_ten[t] : m->ten_d;
                 float f = 0.f;
-                if (len > m->ten_range[t][1]) f = -m->ten_k * (len - m->ten_range[t][1]) - m->ten_d * rate;
-                else if (len < m->ten_range[t][0]) f = -m->ten_k * (len - m->ten_range[t][0]) - m->ten_d * rate;
+                if (len > m->ten_range[t][1]) f = -m->ten_k * (len - m->ten_range[t][1]) - td * rate;
+                else if (len < m->ten_range[t][0]) f = -m->ten_k * (len - m->ten_range[t][0]) - td * rate;
                 if ((r0 >> 8) == lane) { float4 u = S4(r0 & 255, 7); u.w = c0 * f; S4(r0 & 255, 7) = u; }
                 if ((r1 >> 8) == lane) { float4 u = S4(r1 & 255, 7); u.w = c1 * f; S4(r1 & 255, 7) = u; }
             }
@@ -851,14 +857,19 @@ struct Stepper {
                     }
                     // joint force: explicit part + implicit diagonal (linear terms at the end of the sub-step)
                     const float qp = q + h * qd;
-                    float jd = lk.damping, jk = lk.stiffness, jlo = lk.lower, jhi = lk.upper;
-                    if (dr_dof) { const float4 v = dr_dof[sr.link - 1]; jd = v.x; jk = v.y; jlo = v.z; jhi = v.w; }
+                    float jd = lk.damping, jk = lk.stiffness, jlo = lk.lower, jhi = lk.upper, kp = lk.kp, kd = lk.kd;
+                    if (dr_dof) {      // a position-driven DOF: all of its velocity damping, and its drive stiffness kp
+                        const float4 v = dr_dof[sr.link - 1];
+                        jd = v.x;
+                        if (lk.flags & LF_POSDRIVE) { kd = 0.f; kp = v.y; } else jk = v.y;
+                        jlo = v.z; jhi = v.w;
+                    }
                     float f = -jd * qd - jk * qp;
                     float dg = lk.armature + h * jd + h * h * jk;
                     if (lk.flags & LF_POSDRIVE) {
-                        float pd = lk.kp * (act - qp) - lk.kd * qd;
+                        float pd = kp * (act - qp) - kd * qd;
                         pd = fminf(fmaxf(pd, -lk.effort), lk.effort);
-                        f += pd; dg += h * lk.kd + h * h * lk.kp;
+                        f += pd; dg += h * kd + h * h * kp;
                     } else {
                         f += fminf(fmaxf(act, -lk.effort), lk.effort);
                     }
@@ -902,6 +913,14 @@ struct Stepper {
     __device__ __forceinline__ void set_obj_force(float fx, float fy, float fz) const {
         if (lane == 0) A4(m->obj_pose_acc, 5) = make_float4(fx, fy, fz, 0.f);
     }
+    // DR: this env's object size scale, mass factor, hand-object friction and object-ground friction, parked in the free row 6
+    // of the pose accumulator like the external force (same publication rule: call before the first substep())
+    __device__ __forceinline__ void set_obj_params(float scale, float mass_factor, float mu_hand_obj, float mu_obj_ground) const {
+        if (lane == 0) A4(m->obj_pose_acc, 6) = make_float4(scale, mass_factor, mu_hand_obj, mu_obj_ground);
+    }
+    __device__ __forceinline__ float4 obj_params() const {
+        return DR ? A4(m->obj_pose_acc, 6) : make_float4(1.f, 1.f, m->obj_mu, m->obj_mu);
+    }
     __device__ __forceinline__ void obj_load_pose(ObjPose &P) const {
         const int ai = m->obj_pose_acc;
         const float4 a = A4(ai, 0), b = A4(ai, 1), c = A4(ai, 2), d = A4(ai, 3), e = A4(ai, 4);
@@ -917,14 +936,17 @@ struct Stepper {
                                                       const float x[3], const float vw[3], const float vl[3],
                                                       float IA[21], float pa[3], float pl[3],
                                                       const float aw[3], const float al[3], float F[3], float T[3]) const {
-        const float h = m->h, gn = m->obj_cn + h * m->obj_kn;
+        // DR: the gains follow the object's mass (object_contact_gains is linear in it), the friction is this env's
+        const float4 op = obj_params();
+        const float okn = DR ? m->obj_kn * op.y : m->obj_kn, ocn = DR ? m->obj_cn * op.y : m->obj_cn;
+        const float h = m->h, gn = ocn + h * okn;
         float wxr[3], oxr[3]; cross(vw, r, wxr); cross(P.w, r, oxr);
         const float rel[3] = {vl[0] + wxr[0] - P.vO[0] - oxr[0], vl[1] + wxr[1] - P.vO[1] - oxr[1], vl[2] + wxr[2] - P.vO[2] - oxr[2]};
         const float un = dot3(rel, n);
-        const float Fn = m->obj_kn * pen - gn * un;
+        const float Fn = okn * pen - gn * un;
         if (Fn <= 0.f) return;
         const float ut[3] = {rel[0] - un * n[0], rel[1] - un * n[1], rel[2] - un * n[2]};
-        const float gam = m->obj_mu * Fn * rsqrtf(dot3(ut, ut) + m->vs2);
+        const float gam = op.z * Fn * rsqrtf(dot3(ut, ut) + m->vs2);
         const float F0[3] = {Fn * n[0] - gam * ut[0], Fn * n[1] - gam * ut[1], Fn * n[2] - gam * ut[2]};
         if (ACCUM) {
             float dM[21];
@@ -968,8 +990,9 @@ struct Stepper {
                                                       const float aw[3], const float al[3], float F[3], float T[3],
                                                       int cp_first, int cp_step) const {
         ObjPose P; obj_load_pose(P);
-        const float hb[3] = {m->obj_half[0], m->obj_half[1], m->obj_half[2]};
-        const float orad = m->obj_round;                   // read once: the sphere loop below is the hot loop of the hand kernels
+        const float os = DR ? obj_params().x : 1.f;        // DR: this env's size scale of the object's contact shape
+        const float hb[3] = {DR ? m->obj_half[0] * os : m->obj_half[0], DR ? m->obj_half[1] * os : m->obj_half[1], DR ? m->obj_half[2] * os : m->obj_half[2]};
+        const float orad = DR ? m->obj_round * os : m->obj_round;   // read once: the sphere loop below is the hot loop of the hand kernels
 #pragma unroll 1
         for (int k = lk.cp_begin + cp_first; k < lk.cp_end; k += cp_step) {
             const CpC &cp = gr.cps[k];
@@ -1023,9 +1046,12 @@ struct Stepper {
 #pragma unroll
             for (int c = 0; c < 3; c++) { pao[c] = t[21 + c]; plo[c] = t[24 + c]; }
         }
-        // corners against the ground plane, dealt round-robin to the lanes
-        const float gn = m->obj_cn + h * m->obj_kn, orad = m->obj_round;
-        const float hbo[3] = {m->obj_half[0], m->obj_half[1], m->obj_half[2]};
+        // corners against the ground plane, dealt round-robin to the lanes.  DR: this env's size scale s, mass factor (mass and
+        // contact gains; inertia x mass factor x s^2) and object-ground friction
+        const float4 op = obj_params();
+        const float okn = DR ? m->obj_kn * op.y : m->obj_kn, ocn = DR ? m->obj_cn * op.y : m->obj_cn;
+        const float gn = ocn + h * okn, orad = DR ? m->obj_round * op.x : m->obj_round;
+        const float hbo[3] = {DR ? m->obj_half[0] * op.x : m->obj_half[0], DR ? m->obj_half[1] * op.x : m->obj_half[1], DR ? m->obj_half[2] * op.x : m->obj_half[2]};
 #pragma unroll 1
         for (int cn = lane; cn < 8; cn += L) {
             if (obj_corner_dup(cn, hbo)) continue;
@@ -1037,9 +1063,9 @@ struct Stepper {
             r[2] -= orad;                                                // contact point: the sphere's lowest point
             float oxr[3]; cross(P.w, r, oxr);
             const float u[3] = {P.vO[0] + oxr[0], P.vO[1] + oxr[1], P.vO[2] + oxr[2]};
-            const float Fn = m->obj_kn * d - gn * u[2];
+            const float Fn = okn * d - gn * u[2];
             if (Fn <= 0.f) continue;
-            const float gam = m->obj_mu * Fn * rsqrtf(u[0] * u[0] + u[1] * u[1] + m->vs2);
+            const float gam = op.w * Fn * rsqrtf(u[0] * u[0] + u[1] * u[1] + m->vs2);
             const float F0[3] = {-gam * u[0], -gam * u[1], Fn}, ez[3] = {0.f, 0.f, 1.f};
             contact_inertia(Io, h, gam, gn, r, ez);
             float rxF[3]; cross(r, F0, rxF);
@@ -1051,7 +1077,8 @@ struct Stepper {
 #pragma unroll
         for (int c = 0; c < 3; c++) { pao[c] = lane_sum<L>(pao[c]); plo[c] = lane_sum<L>(plo[c]); }
         {   // rigid-body terms about O: Icw = Ro diag(I) Ro^T
-            const float *Ro = P.Ro, i0 = m->obj_I[0], i1 = m->obj_I[1], i2 = m->obj_I[2];
+            const float isc = DR ? op.y * (op.x * op.x) : 1.f;
+            const float *Ro = P.Ro, i0 = DR ? m->obj_I[0] * isc : m->obj_I[0], i1 = DR ? m->obj_I[1] * isc : m->obj_I[1], i2 = DR ? m->obj_I[2] * isc : m->obj_I[2];
             float Icw[6];
             Icw[0] = i0 * Ro[0] * Ro[0] + i1 * Ro[1] * Ro[1] + i2 * Ro[2] * Ro[2];
             Icw[1] = i0 * Ro[3] * Ro[3] + i1 * Ro[4] * Ro[4] + i2 * Ro[5] * Ro[5];
@@ -1059,9 +1086,10 @@ struct Stepper {
             Icw[3] = i0 * Ro[0] * Ro[3] + i1 * Ro[1] * Ro[4] + i2 * Ro[2] * Ro[5];
             Icw[4] = i0 * Ro[0] * Ro[6] + i1 * Ro[1] * Ro[7] + i2 * Ro[2] * Ro[8];
             Icw[5] = i0 * Ro[3] * Ro[6] + i1 * Ro[4] * Ro[7] + i2 * Ro[5] * Ro[8];
-            const float go[3] = {m->obj_g[0], m->obj_g[1], m->obj_g[2]};
+            const float *gsrc = (DR && dr_grav && m->obj_gravity_on) ? dr_grav : m->obj_g;
+            const float go[3] = {gsrc[0], gsrc[1], gsrc[2]};
             float I[21], qa[3], ql[3];
-            spatial_inertia(m->obj_mass, 1.f, Icw, P.c, P.w, P.vO, go, I, qa, ql, m->obj_ang_damp, m->obj_lin_damp);
+            spatial_inertia(DR ? m->obj_mass * op.y : m->obj_mass, 1.f, Icw, P.c, P.w, P.vO, go, I, qa, ql, m->obj_ang_damp, m->obj_lin_damp);
 #pragma unroll
             for (int c = 0; c < 21; c++) Io[c] += I[c];
 #pragma unroll
@@ -1111,7 +1139,8 @@ struct Stepper {
     __device__ __forceinline__ void substep(RootState &rs, const bool LAST, const Outputs &o, ObjState *ob = nullptr) const {
         const float h = m->h;
         const int NS = m->ns;
-        const float g[3] = {m->g[0], m->g[1], m->g[2]};
+        const float *gsrc = (DR && dr_grav && m->gravity_on) ? dr_grav : m->g;
+        const float g[3] = {gsrc[0], gsrc[1], gsrc[2]};
         const bool fixed = m->root_fixed != 0;
 
         pass1(rs);

@@ -81,7 +81,8 @@ __device__ __forceinline__ void hand_force_update(const b2g_hand_params &P, uint
     }
 }
 
-template <int L, int BLOCK>
+// DR: the instantiation that reads the per-env object, tendon and gravity parameters (b200gym.cu attach_object_params)
+template <int L, int BLOCK, bool DR = false>
 __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__restrict__ gm, Buffers B,
                                                           const __grid_constant__ b2g_hand_params P,
                                                           const __grid_constant__ HandDev H,
@@ -89,15 +90,16 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
     prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
-    using ST = Stepper<L, false, BLOCK, true>;
+    using ST = Stepper<L, false, BLOCK, true, false, DR>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;
     const bool valid = env < N;
     const int e = valid ? env : N - 1;
     const bool w0 = valid && lane == 0;
     const int nd = sm.nl - 1, NS = sm.ns, NA = P.num_actions, O = P.num_obs;
-    ST st = make_stepper<L, false, BLOCK, true>(&sm, nullptr, lane);
+    ST st = make_stepper<L, false, BLOCK, true, false, DR>(&sm, nullptr, lane);
     attach_env_params_generic(st, sm, B, e);                 // per-env link masses / joint properties / friction, when bound
+    if (DR) attach_object_params(st, sm, B, e);             // object size / mass / friction, tendon damping, gravity
 
     float *const rows = (float *)B.p[B2G_T_ROOT_STATE] + (size_t)e * 39;          // hand | object | goal marker
     const float *const init_rows = (const float *)B.p[B2G_T_INITIAL_ROOT] + (size_t)e * 39;

@@ -23,7 +23,7 @@ MAXL = 32
  T_FEET_AIR_TIME, T_TORQUES, T_EPISODE_SUMS, T_TERRAIN_LEVELS, T_TERRAIN_TYPES, T_ENV_ORIGINS, T_TERRAIN_ORIGINS,
  T_NOISE_SCALE, T_BASE_SCRATCH, T_REDUCE_SCRATCH, T_ENV_FRICTION, T_GOAL_STATES, T_PREV_TARGETS, T_SUCCESSES,
  T_CONSECUTIVE_SUCCESSES, T_RESET_GOAL, T_GOAL_RESET_COUNT, T_STATES, T_ENV_MASS_SCALE, T_ENV_DOF_PROPS,
- T_JACOBIAN, T_MASS_MATRIX, T_OBJ_FORCE, T_RANDOM_FORCE_PROB) = range(48)
+ T_JACOBIAN, T_MASS_MATRIX, T_OBJ_FORCE, T_RANDOM_FORCE_PROB, T_ENV_OBJ_PROPS, T_ENV_TENDON_DAMPING, T_GRAVITY) = range(51)
 TASK_NONE, TASK_CARTPOLE, TASK_ANT, TASK_HUMANOID, TASK_ANYMAL_TERRAIN, TASK_SHADOW_HAND = 0, 1, 2, 3, 4, 5
 HAND_OBS = {"openai": 0, "full_no_vel": 1, "full": 2, "full_state": 3}
 

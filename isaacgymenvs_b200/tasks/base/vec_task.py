@@ -141,13 +141,15 @@ class VecTask(Env):
         self.viewer = None
         self.first_randomization = True
         self.dr_randomizations = {}
-        # domain randomisation: observation / action noise only (utils/dr.py); physical parameters raise
+        # domain randomisation (utils/dr.py): observation / action noise, gravity where the task's kernels read it, and the
+        # physical actor parameters below
         self.randomizer = None
         task_cfg = self.cfg.get("task", {}) if isinstance(self.cfg, dict) else {}
         self.physical_randomizer = None
         if task_cfg.get("randomize", False):
             from ...utils.dr import Randomizer
-            self.randomizer = Randomizer(task_cfg.get("randomization_params", {}))
+            self.randomizer = Randomizer(task_cfg.get("randomization_params", {}),
+                                         gravity=tuple(sim_cfg["gravity"]) if self.dr_gravity else None, device=self.device)
         if self.device == "cpu":
             raise engine.EngineError(
                 "sim_device=cpu / pipeline=cpu: the CUDA-native stepper has no CPU path (north_star: no CPU "
@@ -165,10 +167,23 @@ class VecTask(Env):
         if ap:      # physical domain randomisation: per-env parameter tensors read by the step kernel (utils/dr.py)
             from ...utils.dr import PhysicalRandomizer
             self.physical_randomizer = PhysicalRandomizer(ap, self.model, self.num_envs, self.device,
-                                                          task_cfg["randomization_params"].get("frequency", 1))
+                                                          task_cfg["randomization_params"].get("frequency", 1), **self._dr_actors())
             self.physical_randomizer.apply(0, self.randomize_buf, self.reset_buf)
             for slot, t in self.physical_randomizer.tensors(engine).items():
                 self.sim._bind(slot, t)
+        if self.randomizer is not None and self.randomizer.gravity is not None:
+            self.sim._bind(engine.T_GRAVITY, self.randomizer.gravity)
+
+    # tasks whose kernels read a bound gravity vector (sim_params.gravity randomisation)
+    dr_gravity = False
+
+    def _dr_actors(self) -> dict:
+        """keyword arguments of PhysicalRandomizer naming the actors of a multi-actor task (default: one articulation)."""
+        return {}
+
+    def _randomize_this_step(self) -> bool:
+        """whether step() runs apply_randomizations before the physics (default: every step)."""
+        return True
 
     # ---- vec_task.py:301-324
     def allocate_buffers(self):
@@ -237,10 +252,12 @@ class VecTask(Env):
 
     # ---- vec_task.py:360-408
     def step(self, actions: torch.Tensor) -> Tuple[Dict[str, torch.Tensor], torch.Tensor, torch.Tensor, Dict[str, Any]]:
+        randomize = (self.physical_randomizer is not None or self.randomizer is not None) and self._randomize_this_step()
         if self.physical_randomizer is not None:   # apply_randomizations for the envs this step is about to reset (vec_task.py:631-637)
-            self.physical_randomizer.apply(self.control_steps * max(int(self.control_freq_inv), 1), self.randomize_buf, self.reset_buf)
+            if randomize:
+                self.physical_randomizer.apply(self.control_steps * max(int(self.control_freq_inv), 1), self.randomize_buf, self.reset_buf)
             self.randomize_buf += 1
-        if self.randomizer is not None:         # apply_randomizations, vec_task.py:610-718 (non-physical part)
+        if self.randomizer is not None and randomize:     # apply_randomizations, vec_task.py:610-718 (non-physical part)
             if self.randomizer.update(self.control_steps * max(int(self.control_freq_inv), 1)):
                 for key, model in self.randomizer.models.items():
                     self.dr_randomizations[key] = {"noise_lambda": model}

@@ -40,7 +40,8 @@ class ShadowHand(VecTask):
         self.cfg = cfg
         e = cfg["env"]
         self.randomize = cfg["task"]["randomize"]
-        # randomize: observation / action noise is applied by the base class; physical randomisation raises there
+        # randomize: the base class applies the noise, gravity and the hand / object actor_params (utils/dr.py), on the steps
+        # that reset some env (reset_idx calls apply_randomizations, shadow_hand.py:604-607,670-682)
         self.dist_reward_scale = e["distRewardScale"]; self.rot_reward_scale = e["rotRewardScale"]
         self.action_penalty_scale = e["actionPenaltyScale"]; self.success_tolerance = e["successTolerance"]
         self.reach_goal_bonus = e["reachGoalBonus"]; self.fall_dist = e["fallDistance"]; self.fall_penalty = e["fallPenalty"]
@@ -109,7 +110,8 @@ class ShadowHand(VecTask):
         model = self._build_model()
         sim_cfg = self.cfg["sim"]
         self.model = model
-        ext = engine.pack_model_ext(model, obj=self._obj, actors_per_env=3, tendons=self._tendons, tendon_k=30.0, tendon_d=0.1)
+        self.tendon_damping = 0.1                                                                              # t_damping, shadow_hand.py:257
+        ext = engine.pack_model_ext(model, obj=self._obj, actors_per_env=3, tendons=self._tendons, tendon_k=30.0, tendon_d=self.tendon_damping)
         self.sim = sim = engine.Sim(model, self.num_envs, dt=sim_cfg["dt"], substeps=sim_cfg["substeps"],
                                     gravity=tuple(sim_cfg["gravity"]), ground_mu=1.0, device=self.device, ext=ext)
         dev, N = self.device, self.num_envs
@@ -168,6 +170,16 @@ class ShadowHand(VecTask):
         self.object_rb_handles = torch.tensor([model.nb], dtype=torch.long, device=dev)
         self.total_successes = 0; self.total_resets = 0
         return sim
+
+    # ---- domain randomisation (task.randomize): the hand and object kernels read per-env object, tendon and gravity parameters
+    dr_gravity = True
+
+    def _dr_actors(self):
+        return dict(actors={"hand": "articulation", "object": "object"}, obj=self._obj,
+                    tendon_damping=[self.tendon_damping] * len(self._tendons))
+
+    def _randomize_this_step(self):
+        return bool(self.reset_buf.any())
 
     @property
     def rigid_body_states(self):
