@@ -322,42 +322,24 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
         const int d = st.link_of(s) - 1;
         if (d < 0) continue;
         float2 qv = st.get_q(s);
-        if (do_reset) {
-            const float up = reset_uniform(P.seed, gid, count, d);
-            const float uv = reset_uniform(P.seed, gid, count, nd + d);
-            const float pos = (P.reset_pos_noise - (-P.reset_pos_noise)) * up + (-P.reset_pos_noise);
-            qv.x = fmaxf(fminf(P.initial_dof_pos[d] + pos, P.dof_limits_upper[d]), P.dof_limits_lower[d]);
-            qv.y = (P.reset_vel_noise - (-P.reset_vel_noise)) * uv + (-P.reset_vel_noise);
-        }
+        if (do_reset) qv = loco_reset_dof(P, gid, count, d, nd);
         if (valid) row_dof[d] = qv;
     }
     if (do_reset) {
-        const float *ir = (const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e;
-        rs.rp[0] = ir[0]; rs.rp[1] = ir[1]; rs.rp[2] = ir[2];
-        rs.rq[0] = ir[3]; rs.rq[1] = ir[4]; rs.rq[2] = ir[5]; rs.rq[3] = ir[6];
-        rs.rv[0] = ir[7]; rs.rv[1] = ir[8]; rs.rv[2] = ir[9];
-        rs.rw[0] = ir[10]; rs.rw[1] = ir[11]; rs.rw[2] = ir[12];
-        potentials = t_potential(P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], P.dt);
+        potentials = loco_reset_root(P, B, e, rs);
         progress = 0;
         if (valid && lane == 0) rc[e] = (int)(count + 1);
     }
     if (valid && lane == 0 && !sm.root_fixed) store_root(row_root, rs);
 
     // the slot state is dead from here on: its shared memory becomes the output staging area
-    // layout (floats unless noted): obs | obs_clipped? | rew | pot | ppot | up(3) | head(3) | reset(i64) | progress(i64) | timeout(u8)
     __syncthreads();
     float *const g_obs = (float *)B.p[B2G_T_OBS];
     float *g_obsc = (float *)B.p[B2G_T_OBS_CLIPPED];
     if (g_obsc == g_obs) g_obsc = nullptr;
-    float *const so = reinterpret_cast<float *>(b2g_dyn_smem);
-    float *const t_obs = so;
-    float *const t_obsc = t_obs + EPB * O;
-    float *const t_rew = t_obsc + (g_obsc ? EPB * O : 0);
-    float *const t_pot = t_rew + EPB, *const t_ppot = t_pot + EPB, *const t_up = t_ppot + EPB, *const t_head = t_up + 3 * EPB;
-    long long *const t_reset = reinterpret_cast<long long *>(t_head + 3 * EPB), *const t_prog = t_reset + EPB;
-    uint8_t *const t_to = reinterpret_cast<uint8_t *>(t_prog + EPB);
-    float *const obs = tiles ? t_obs + (size_t)el * O : g_obs + (size_t)e * O;
-    float *const obsc = g_obsc ? (tiles ? t_obsc + (size_t)el * O : g_obsc + (size_t)e * O) : nullptr;
+    const LocoStage t = loco_stage(reinterpret_cast<float *>(b2g_dyn_smem), EPB, O, g_obsc != nullptr);
+    float *const obs = tiles ? t.obs + (size_t)el * O : g_obs + (size_t)e * O;
+    float *const obsc = g_obsc ? (tiles ? t.obsc + (size_t)el * O : g_obsc + (size_t)e * O) : nullptr;
 
     // compute_observations
     LocoRootObs ro;
@@ -379,7 +361,7 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     const int o_pos = 12, o_vel = 12 + nd, o_frc = 12 + 2 * nd;
     const int o_sens = HUM ? 12 + 3 * nd : 12 + 2 * nd;
     const int o_act = o_sens + nsens6;
-    float actions_cost = 0.f, electricity = 0.f, at_limit = 0.f;
+    LocoCosts cost;
 #pragma unroll 1
     for (int s = 0; s < NS; s++) {
         const int link = st.link_of(s), d = link - 1;
@@ -395,45 +377,27 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
 #pragma unroll
             for (int c = 0; c < 6; c++) put(o_sens + 6 * sk + c, o.sensor[6 * sk + c] * P.contact_force_scale);
         }
-        // compute_ant_reward (ant.py:353-355) / compute_humanoid_reward (humanoid.py:352-359)
-        actions_cost += a * a;
-        if (HUM) {
-            const float ratio = P.motor_efforts[d] / P.max_motor_effort;
-            const float scaled = P.joints_at_limit_cost_scale * (fabsf(ps) - 0.98f) / 0.02f;
-            at_limit += (fabsf(ps) > 0.98f) ? scaled * ratio : 0.f;
-            electricity += fabsf(a * vs) * ratio;
-        } else {
-            at_limit += (ps > 0.99f) ? 1.f : 0.f;
-            electricity += fabsf(a * vs);
-        }
+        cost.add(P, d, a, ps, vs, HUM);
     }
     if (lane == 0 && st.links[0].sensor >= 0 && o.sensor) {
         const int sk = st.links[0].sensor;
 #pragma unroll
         for (int c = 0; c < 6; c++) put(o_sens + 6 * sk + c, o.sensor[6 * sk + c] * P.contact_force_scale);
     }
-    actions_cost = lane_sum<L>(actions_cost);
-    electricity = lane_sum<L>(electricity);
-    at_limit = lane_sum<L>(at_limit);
+    cost.sum_lanes<L>();
 
     if (valid && lane == 0) {
-        const float heading_proj = ro.o[11], up_proj = ro.o[10], height = ro.o[0];
-        const float heading_reward = (heading_proj > 0.8f) ? P.heading_weight : P.heading_weight * heading_proj / 0.8f;
-        const float up_reward = (up_proj > 0.93f) ? P.up_weight : 0.f;
-        const float progress_reward = potentials - prev_potentials;
-        float total_r = progress_reward + P.alive_reward + up_reward + heading_reward - P.actions_cost_scale * actions_cost -
-                        P.energy_cost_scale * electricity - (HUM ? at_limit : at_limit * P.joints_at_limit_cost_scale);
-        long long reset = 0;                       // reset_buf was cleared by reset_idx or was already 0
-        if (height < P.termination_height) { total_r = P.death_cost; reset = 1; }
-        if ((float)progress >= P.max_episode_length - 1.f) reset = 1;
-        const uint8_t tout = (uint8_t)(((float)progress >= P.max_episode_length - 1.f) && reset != 0);   // vec_task.py:394
+        const LocoReward r = loco_reward(P, ro.o[10], ro.o[11], potentials, prev_potentials, cost, ro.o[0], progress, HUM);
+        const float total_r = r.rew;
+        const long long reset = (r.died || r.timed) ? 1 : 0;
+        const uint8_t tout = r.timed;
         float *uv = (float *)B.p[B2G_T_UP_VEC], *hv = (float *)B.p[B2G_T_HEADING_VEC];
         uint8_t *to = (uint8_t *)B.p[B2G_T_TIMEOUT];
         if (tiles) {
-            t_rew[el] = total_r; t_reset[el] = reset; t_prog[el] = progress; t_pot[el] = potentials; t_ppot[el] = prev_potentials;
-            t_up[3 * el] = ro.up_vec[0]; t_up[3 * el + 1] = ro.up_vec[1]; t_up[3 * el + 2] = ro.up_vec[2];
-            t_head[3 * el] = ro.heading_vec[0]; t_head[3 * el + 1] = ro.heading_vec[1]; t_head[3 * el + 2] = ro.heading_vec[2];
-            t_to[el] = tout;
+            t.rew[el] = total_r; t.reset[el] = reset; t.prog[el] = progress; t.pot[el] = potentials; t.ppot[el] = prev_potentials;
+            t.up[3 * el] = ro.up_vec[0]; t.up[3 * el + 1] = ro.up_vec[1]; t.up[3 * el + 2] = ro.up_vec[2];
+            t.head[3 * el] = ro.heading_vec[0]; t.head[3 * el + 1] = ro.heading_vec[1]; t.head[3 * el + 2] = ro.heading_vec[2];
+            t.to[el] = tout;
         } else {
             ((float *)B.p[B2G_T_REW])[e] = total_r;
             reset_b[e] = reset; progress_b[e] = progress;
@@ -453,31 +417,20 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
             if (g_act_out) bulk_s2g(g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
             if (stage_out && g_sens && nsens6) bulk_s2g(g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
             if (stage_out && HUM && g_dfrc) bulk_s2g(g_dfrc + e0 * nd, s_dfrc, (uint32_t)(EPB * nd * 4));
-            bulk_s2g(g_obs + e0 * O, t_obs, (uint32_t)(EPB * O * 4));
-            if (g_obsc) bulk_s2g(g_obsc + e0 * O, t_obsc, (uint32_t)(EPB * O * 4));
-            bulk_s2g((float *)B.p[B2G_T_REW] + e0, t_rew, EPB * 4);
-            bulk_s2g(pot_b + e0, t_pot, EPB * 4);
-            bulk_s2g(ppot_b + e0, t_ppot, EPB * 4);
-            if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, t_up, EPB * 12);
-            if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t_head, EPB * 12);
-            bulk_s2g(reset_b + e0, t_reset, EPB * 8);
-            bulk_s2g(progress_b + e0, t_prog, EPB * 8);
-            if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t_to, EPB);
+            bulk_s2g(g_obs + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
+            if (g_obsc) bulk_s2g(g_obsc + e0 * O, t.obsc, (uint32_t)(EPB * O * 4));
+            bulk_s2g((float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
+            bulk_s2g(pot_b + e0, t.pot, EPB * 4);
+            bulk_s2g(ppot_b + e0, t.ppot, EPB * 4);
+            if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, t.up, EPB * 12);
+            if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t.head, EPB * 12);
+            bulk_s2g(reset_b + e0, t.reset, EPB * 8);
+            bulk_s2g(progress_b + e0, t.prog, EPB * 8);
+            if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
 
             bulk_commit_wait();
         }
-        // host copies of what VecTask.step returns (vec_task.py:402-408), straight over PCIe: coalesced 16-byte stores
-        if (HOSTIO) {
-            const size_t e0 = (size_t)env0;
-            auto copy16 = [&](void *dst, const void *src, int bytes) {
-                float4 *d = reinterpret_cast<float4 *>(dst); const float4 *sp = reinterpret_cast<const float4 *>(src);
-                for (int i = threadIdx.x; i < bytes / 16; i += BLOCK) d[i] = sp[i];
-            };
-            if (ta.h_obs) copy16(ta.h_obs + e0 * O, g_obsc ? t_obsc : t_obs, EPB * O * 4);
-            if (ta.h_rew) copy16(ta.h_rew + e0, t_rew, EPB * 4);
-            if (ta.h_reset) copy16(ta.h_reset + e0, t_reset, EPB * 8);
-            if (ta.h_timeout) copy16(ta.h_timeout + e0, t_to, EPB);
-        }
+        if (HOSTIO) loco_copy_to_host<BLOCK>(ta, t, (size_t)env0, EPB, O, g_obsc != nullptr);
     }
 }
 
@@ -1127,13 +1080,11 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
     const bool hum = P.task == B2G_TASK_HUMANOID;
     const int O = P.num_obs, ns6 = 6 * s->hm.nsens;
     const bool clip_sep = s->buf.p[B2G_T_OBS_CLIPPED] && s->buf.p[B2G_T_OBS_CLIPPED] != s->buf.p[B2G_T_OBS];
-    // the output tiles, staged in the shared memory of the slot state: obs | obs_clipped? | rew | pot | ppot | up | head | reset | progress | timeout
-    auto out_bytes = [&](int epb) { return (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1); };
     if (!hum && s->quad_ns == 2 && !s->d_hf) {           // Ant on the quad sub-step (whole tiles only)
         constexpr int EPB = QUAD_LOCO_BLOCK / 4, ND = 8;
         const size_t park_bytes = (size_t)quad_park_f4(2) * QUAD_LOCO_BLOCK * sizeof(float4);
         const size_t io_bytes = ((size_t)EPB * (13 + 3 * ND + ns6) * 4 + 15) & ~(size_t)15;
-        if (whole_tiles(N, EPB) && out_bytes(EPB) <= park_bytes) {
+        if (whole_tiles(N, EPB) && loco_stage_bytes(EPB, O, clip_sep) <= park_bytes) {
             const size_t dyn = park_bytes + io_bytes + (size_t)quad_model_f4(2) * sizeof(float4);
             const bool lean = !s->buf.p[B2G_T_ENV_MASS_SCALE] && !s->buf.p[B2G_T_ENV_DOF_PROPS] && !s->buf.p[B2G_T_ENV_FRICTION] &&
                               !s->buf.p[B2G_T_NET_CONTACT] && !s->buf.p[B2G_T_DOF_FORCE];
@@ -1147,7 +1098,7 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
     const int epb = blk / s->lanes, ndof = s->hm.nl - 1;
     const size_t state_bytes = s->dyn_smem;                                   // slot state + accumulators
     const size_t io_bytes = ((size_t)epb * (13 + 3 * ndof + ns6 + (hum ? ndof : 0)) * 4 + 15) & ~(size_t)15;
-    const bool tiles = whole_tiles(N, epb) && out_bytes(epb) <= state_bytes && s->buf.p[B2G_T_ACTIONS];
+    const bool tiles = whole_tiles(N, epb) && loco_stage_bytes(epb, O, clip_sep) <= state_bytes && s->buf.p[B2G_T_ACTIONS];
     const size_t model_bytes = offsetof(DevModel, slots) + (size_t)s->hm.ns * MAX_LANES * sizeof(SlotRec) + (((size_t)s->hm.nl * sizeof(LinkC) + 15) & ~(size_t)15) +
                                (((size_t)s->hm.ncp * sizeof(CpC) + 15) & ~(size_t)15);
     const size_t io_used = tiles ? io_bytes : 16;
@@ -1235,8 +1186,8 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     const size_t park_f4 = (size_t)quad_park_f4(2) * QB;
     const size_t io_f4 = ((size_t)EPB * (13 + 2 * nd_ + 2 * nd_ + ns6) * 4 + 15) / 16;
     const size_t model_f4 = quad_model_f4(2);
-    const size_t stage_f4 = ((size_t)EPB * (O * 4 + 4 + 8 + 1) + 15) / 16;
-    if ((size_t)EPB * (O * 4 + 4 * 2 + 12 * 2 + 8) > park_f4 * 16) return fail(B2G_E_UNSUPPORTED, "b2g_task_rollout: observation too large for the last-step staging");
+    const size_t stage_f4 = (roll_stage_bytes(EPB, O) + 15) / 16;
+    if (roll_last_bytes(EPB, O) > park_f4 * 16) return fail(B2G_E_UNSUPPORTED, "b2g_task_rollout: observation too large for the last-step staging");
     RollArgs ra;
     ra.actions = actions; ra.obs_out = obs_out; ra.rew_out = rew_out; ra.reset_out = (long long *)reset_out; ra.timeout_out = timeout_out;
     ra.K = K; ra.io_f4 = (int)park_f4; ra.model_f4 = (int)(park_f4 + io_f4); ra.stage_f4 = (int)(park_f4 + io_f4 + model_f4);

@@ -70,6 +70,91 @@ __global__ void __launch_bounds__(BLOCK) quad_simulate_kernel(const float4 *__re
 }
 
 // -------------------------------------------------------------------------------------------
+// compute_observations of Ant (ant.py:374-408) on the four lanes of env e, with the per-DOF sums of its reward (summed on
+// this lane only).  put(idx, v) stores element idx of the observation; lane 0 also returns the up / heading vectors and
+// projections.  The sensor rows come from the staged tile row s_row after a simulate (stage_out), else from the tensor.
+struct AntRootObs {
+    float up_proj = 0.f, heading_proj = 0.f;
+    float up_vec[3], heading_vec[3];
+};
+template <int NS, class PUT>
+__device__ __forceinline__ LocoCosts ant_obs(const b2g_task_params &P, const RootState &rs, const float (&q)[NS], const float (&qd)[NS],
+                                             const int (&dofi)[NS], const int (&sens)[NS], const float (&a_cl)[NS], const float4 *qm, int lane,
+                                             const float *s_sens, const float *g_sens, int e, int el, int nsens6, bool stage_out, AntRootObs &ro, PUT put) {
+    constexpr int nd = 4 * NS;
+    // The three Euler / heading angles are three atan2f calls on different arguments: the lanes of the env take one each
+    // (same instruction stream, different data) and hand it to lane 0.
+    const float to_t[3] = {P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], 0.f};
+    const float isr[4] = {-0.f, -0.f, -0.f, 1.f};
+    float tq[4]; t_quat_mul(rs.rq, isr, tq);                   // compute_heading_and_up, torch_jit_utils.py:247-262
+    float ang_mine;
+    {
+        const float qx = tq[0], qy = tq[1], qz = tq[2], qw = tq[3];
+        // get_euler_xyz :175-195 (roll, yaw) and compute_rot :265-276 (walk_target_angle); lane 3 duplicates lane 0
+        const float ay = (lane == 1) ? 2.0f * (qw * qx + qy * qz) : (lane == 2) ? P.target[2] - rs.rp[2] : 2.0f * (qw * qz + qx * qy);
+        const float ax = (lane == 1) ? qw * qw - qx * qx - qy * qy + qz * qz : (lane == 2) ? P.target[0] - rs.rp[0] : qw * qw + qx * qx - qy * qy - qz * qz;
+        const float a = atan2f(ay, ax);
+        // torch.remainder(a, 2 pi) for a in [-pi, pi] (fmod leaves such an `a` unchanged); the walk angle is not wrapped
+        ang_mine = (lane != 2 && a < 0.f) ? a + 6.2831855f : a;
+    }
+    const float roll = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 1);
+    const float walk = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 2);
+    const float yaw = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28));
+    if (lane == 0) {
+        const float nrm = fmaxf(sqrtf(to_t[0] * to_t[0] + to_t[1] * to_t[1] + 0.f), 1e-9f);
+        const float td[3] = {to_t[0] / nrm, to_t[1] / nrm, 0.f / nrm};
+        const float b0[3] = {1.f, 0.f, 0.f}, b1[3] = {0.f, 0.f, 1.f};
+        t_quat_rotate(tq, b1, ro.up_vec, 1.f);
+        t_quat_rotate(tq, b0, ro.heading_vec, 1.f);
+        ro.up_proj = ro.up_vec[2];
+        ro.heading_proj = (ro.heading_vec[0] * td[0] + ro.heading_vec[1] * td[1]) + ro.heading_vec[2] * td[2];
+        float vloc[3], wloc[3];
+        t_quat_rotate(tq, rs.rv, vloc, -1.f);
+        t_quat_rotate(tq, rs.rw, wloc, -1.f);
+        put(0, rs.rp[2]);
+        put(1, vloc[0]); put(2, vloc[1]); put(3, vloc[2]);
+        put(4, wloc[0]); put(5, wloc[1]); put(6, wloc[2]);
+        put(7, yaw); put(8, roll); put(9, walk - yaw); put(10, ro.up_proj); put(11, ro.heading_proj);
+    }
+    // layout: ant.py:401-406  [12 | nd pos | nd vel | 6*nsens sensors | nd actions]
+    const int o_pos = 12, o_vel = 12 + nd, o_sens = 12 + 2 * nd, o_act = o_sens + nsens6;
+    LocoCosts cost;
+#pragma unroll
+    for (int s = 0; s < NS; s++) {
+        const int d = dofi[s];
+        const float a = a_cl[s];
+        const float ps = t_unscale(q[s], P.dof_limits_lower[d], P.dof_limits_upper[d]);
+        const float vs = qd[s] * P.dof_vel_scale;
+        put(o_pos + d, ps); put(o_vel + d, vs); put(o_act + d, a);
+        if (sens[s] >= 0) {                                    // typed pointers: shared-memory loads of the staged tile, not generic ones
+            float sv[6];
+            if (stage_out) {
+                const float *sp_ = s_sens + nsens6 * el + 6 * sens[s];
+#pragma unroll
+                for (int c = 0; c < 6; c++) sv[c] = sp_[c];
+            } else {                                           // no simulate: the tensor as it stands (golden-vector mode)
+#pragma unroll
+                for (int c = 0; c < 6; c++) sv[c] = g_sens ? g_sens[(size_t)e * nsens6 + 6 * sens[s] + c] : 0.f;
+            }
+            if (stage_out || g_sens) {
+#pragma unroll
+                for (int c = 0; c < 6; c++) put(o_sens + 6 * sens[s] + c, sv[c] * P.contact_force_scale);
+            }
+        }
+        cost.add(P, d, a, ps, vs, false);
+    }
+    {
+        const int rsens = q_f2i(qm[3].w);                      // a sensor on the base itself (not Ant): through the tensor
+        const float *sp_ = stage_out ? s_sens + nsens6 * el : (g_sens ? g_sens + (size_t)e * nsens6 : nullptr);
+        if (lane == 0 && rsens >= 0 && sp_) {
+#pragma unroll
+            for (int c = 0; c < 6; c++) put(o_sens + 6 * rsens + c, sp_[6 * rsens + c] * P.contact_force_scale);
+        }
+    }
+    return cost;
+}
+
+// -------------------------------------------------------------------------------------------
 // One whole VecTask.step() of Ant on the quad sub-step.  Same data movement as loco_step_kernel: every tensor of
 // the step is ONE bulk-async (TMA) copy per block in and out; whole tiles only (the host falls back to
 // loco_step_kernel otherwise).
@@ -174,16 +259,10 @@ __global__ void __launch_bounds__(BLOCK, B2G_QUAD_MINBLOCKS(BLOCK)) quad_loco_ke
         const uint32_t gid = (uint32_t)(e + P.env_id_offset);
 #pragma unroll
         for (int s = 0; s < NS; s++) {
-            const int d = dofi[s];
-            const float up = reset_uniform(P.seed, gid, count, d);
-            const float uv = reset_uniform(P.seed, gid, count, nd + d);
-            const float pos = (P.reset_pos_noise - (-P.reset_pos_noise)) * up + (-P.reset_pos_noise);
-            L.q[s] = fmaxf(fminf(P.initial_dof_pos[d] + pos, P.dof_limits_upper[d]), P.dof_limits_lower[d]);
-            L.qd[s] = (P.reset_vel_noise - (-P.reset_vel_noise)) * uv + (-P.reset_vel_noise);
+            const float2 qv = loco_reset_dof(P, gid, count, dofi[s], nd);
+            L.q[s] = qv.x; L.qd[s] = qv.y;
         }
-        const float *ir = (const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e;
-        load_root(ir, rs);
-        potentials = t_potential(P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], P.dt);
+        potentials = loco_reset_root(P, B, e, rs);
         progress = 0;
         if (lane == 0) rc[e] = (int)(count + 1);
     }
@@ -192,168 +271,68 @@ __global__ void __launch_bounds__(BLOCK, B2G_QUAD_MINBLOCKS(BLOCK)) quad_loco_ke
     if (lane == 0) store_root(row_root, rs);
 
     // the parking area is dead from here on: it becomes the output staging area
-    // layout (floats unless noted): obs | obs_clipped? | rew | pot | ppot | up(3) | head(3) | reset(i64) | progress(i64) | timeout(u8)
     __syncthreads();
     float *const g_obs = (float *)B.p[B2G_T_OBS];
     float *g_obsc = (float *)B.p[B2G_T_OBS_CLIPPED];
     if (g_obsc == g_obs) g_obsc = nullptr;
-    float *const t_obs = reinterpret_cast<float *>(b2g_dyn_smem);
-    float *const t_obsc = t_obs + EPB * O;
-    float *const t_rew = t_obsc + (g_obsc ? EPB * O : 0);
-    float *const t_pot = t_rew + EPB, *const t_ppot = t_pot + EPB, *const t_up = t_ppot + EPB, *const t_head = t_up + 3 * EPB;
-    long long *const t_reset = reinterpret_cast<long long *>(t_head + 3 * EPB), *const t_prog = t_reset + EPB;
-    uint8_t *const t_to = reinterpret_cast<uint8_t *>(t_prog + EPB);
-    float *const obs = t_obs + (size_t)el * O;
-    float *const obsc = g_obsc ? t_obsc + (size_t)el * O : nullptr;
+    const LocoStage t = loco_stage(reinterpret_cast<float *>(b2g_dyn_smem), EPB, O, g_obsc != nullptr);
+    float *const obs = t.obs + (size_t)el * O;
+    float *const obsc = g_obsc ? t.obsc + (size_t)el * O : nullptr;
 
-    // compute_observations (ant.py:374-408).  The three Euler / heading angles are three atan2f calls on different
-    // arguments: the lanes of the env take one each (same instruction stream, different data) and hand it to lane 0.
-    const float to_t[3] = {P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], 0.f};
+    // compute_observations (ant.py:374-408)
     const float prev_potentials = potentials;                  // prev_potentials_new = potentials.clone(), ant.py:390
-    potentials = t_potential(to_t[0], to_t[1], P.dt);
-    const float isr[4] = {-0.f, -0.f, -0.f, 1.f};
-    float tq[4]; t_quat_mul(rs.rq, isr, tq);                   // compute_heading_and_up, torch_jit_utils.py:247-262
-    float ang_mine;
-    {
-        const float qx = tq[0], qy = tq[1], qz = tq[2], qw = tq[3];
-        // get_euler_xyz :175-195 (roll, yaw) and compute_rot :265-276 (walk_target_angle); lane 3 duplicates lane 0
-        const float ay = (lane == 1) ? 2.0f * (qw * qx + qy * qz) : (lane == 2) ? P.target[2] - rs.rp[2] : 2.0f * (qw * qz + qx * qy);
-        const float ax = (lane == 1) ? qw * qw - qx * qx - qy * qy + qz * qz : (lane == 2) ? P.target[0] - rs.rp[0] : qw * qw + qx * qx - qy * qy - qz * qz;
-        const float a = atan2f(ay, ax);
-        // torch.remainder(a, 2 pi) for a in [-pi, pi] (fmod leaves such an `a` unchanged); the walk angle is not wrapped
-        ang_mine = (lane != 2 && a < 0.f) ? a + 6.2831855f : a;
-    }
-    const float roll = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 1);
-    const float walk = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 2);
-    const float yaw = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28));
+    potentials = loco_potential(P, rs.rp);
     const float clipo = P.clip_obs;
-    auto put = [&](int idx, float v) {
-        obs[idx] = v;
-        if (obsc) obsc[idx] = fminf(fmaxf(v, -clipo), clipo);
-    };
-    float up_proj = 0.f, heading_proj = 0.f;
-    float up_vec[3], heading_vec[3];
+    AntRootObs ro;
+    LocoCosts cost = ant_obs<NS>(P, rs, L.q, L.qd, dofi, sens, a_cl, qm, lane, s_sens, g_sens, e, el, nsens6, stage_out, ro,
+                                 [&](int idx, float v) {
+                                     obs[idx] = v;
+                                     if (obsc) obsc[idx] = fminf(fmaxf(v, -clipo), clipo);
+                                 });
+    cost.sum_lanes<4>();
     if (lane == 0) {
-        const float nrm = fmaxf(sqrtf(to_t[0] * to_t[0] + to_t[1] * to_t[1] + 0.f), 1e-9f);
-        const float td[3] = {to_t[0] / nrm, to_t[1] / nrm, 0.f / nrm};
-        const float b0[3] = {1.f, 0.f, 0.f}, b1[3] = {0.f, 0.f, 1.f};
-        t_quat_rotate(tq, b1, up_vec, 1.f);
-        t_quat_rotate(tq, b0, heading_vec, 1.f);
-        up_proj = up_vec[2];
-        heading_proj = (heading_vec[0] * td[0] + heading_vec[1] * td[1]) + heading_vec[2] * td[2];
-        float vloc[3], wloc[3];
-        t_quat_rotate(tq, rs.rv, vloc, -1.f);
-        t_quat_rotate(tq, rs.rw, wloc, -1.f);
-        put(0, rs.rp[2]);
-        put(1, vloc[0]); put(2, vloc[1]); put(3, vloc[2]);
-        put(4, wloc[0]); put(5, wloc[1]); put(6, wloc[2]);
-        put(7, yaw); put(8, roll); put(9, walk - yaw); put(10, up_proj); put(11, heading_proj);
-    }
-    // layout: ant.py:401-406  [12 | nd pos | nd vel | 6*nsens sensors | nd actions]
-    const int o_pos = 12, o_vel = 12 + nd, o_sens = 12 + 2 * nd, o_act = o_sens + nsens6;
-    float actions_cost = 0.f, electricity = 0.f, at_limit = 0.f;
-#pragma unroll
-    for (int s = 0; s < NS; s++) {
-        const int d = dofi[s];
-        const float a = a_cl[s];
-        const float ps = t_unscale(L.q[s], P.dof_limits_lower[d], P.dof_limits_upper[d]);
-        const float vs = L.qd[s] * P.dof_vel_scale;
-        put(o_pos + d, ps); put(o_vel + d, vs); put(o_act + d, a);
-        if (sens[s] >= 0) {                                    // typed pointers: shared-memory loads of the staged tile, not generic ones
-            float sv[6];
-            if (stage_out) {
-                const float *sp_ = s_sens + nsens6 * el + 6 * sens[s];
-#pragma unroll
-                for (int c = 0; c < 6; c++) sv[c] = sp_[c];
-            } else {                                           // no simulate: the tensor as it stands (golden-vector mode)
-#pragma unroll
-                for (int c = 0; c < 6; c++) sv[c] = g_sens ? g_sens[(size_t)e * nsens6 + 6 * sens[s] + c] : 0.f;
-            }
-            if (stage_out || g_sens) {
-#pragma unroll
-                for (int c = 0; c < 6; c++) put(o_sens + 6 * sens[s] + c, sv[c] * P.contact_force_scale);
-            }
-        }
-        actions_cost += a * a;                                 // compute_ant_reward, ant.py:353-355
-        at_limit += (ps > 0.99f) ? 1.f : 0.f;
-        electricity += fabsf(a * vs);
-    }
-    {
-        const int rsens = q_f2i(qm[3].w);                      // a sensor on the base itself (not Ant): through the tensor
-        const float *sp_ = stage_out ? s_sens + nsens6 * el : (g_sens ? g_sens + (size_t)e * nsens6 : nullptr);
-        if (lane == 0 && rsens >= 0 && sp_) {
-#pragma unroll
-            for (int c = 0; c < 6; c++) put(o_sens + 6 * rsens + c, sp_[6 * rsens + c] * P.contact_force_scale);
-        }
-    }
-    actions_cost = lane_sum<4>(actions_cost);
-    electricity = lane_sum<4>(electricity);
-    at_limit = lane_sum<4>(at_limit);
-    if (lane == 0) {
-        const float height = rs.rp[2];
-        const float heading_reward = (heading_proj > 0.8f) ? P.heading_weight : P.heading_weight * heading_proj / 0.8f;
-        const float up_reward = (up_proj > 0.93f) ? P.up_weight : 0.f;
-        const float progress_reward = potentials - prev_potentials;
-        float total_r = progress_reward + P.alive_reward + up_reward + heading_reward - P.actions_cost_scale * actions_cost -
-                        P.energy_cost_scale * electricity - at_limit * P.joints_at_limit_cost_scale;
-        long long reset = 0;
-        if (height < P.termination_height) { total_r = P.death_cost; reset = 1; }
-        if ((float)progress >= P.max_episode_length - 1.f) reset = 1;
-        const uint8_t tout = (uint8_t)(((float)progress >= P.max_episode_length - 1.f) && reset != 0);   // vec_task.py:394
-        t_rew[el] = total_r; t_reset[el] = reset; t_prog[el] = progress; t_pot[el] = potentials; t_ppot[el] = prev_potentials;
-        t_up[3 * el] = up_vec[0]; t_up[3 * el + 1] = up_vec[1]; t_up[3 * el + 2] = up_vec[2];
-        t_head[3 * el] = heading_vec[0]; t_head[3 * el + 1] = heading_vec[1]; t_head[3 * el + 2] = heading_vec[2];
-        t_to[el] = tout;
+        const LocoReward r = loco_reward(P, ro.up_proj, ro.heading_proj, potentials, prev_potentials, cost, rs.rp[2], progress, false);
+        t.rew[el] = r.rew; t.reset[el] = (r.died || r.timed) ? 1 : 0; t.prog[el] = progress; t.pot[el] = potentials; t.ppot[el] = prev_potentials;
+        t.up[3 * el] = ro.up_vec[0]; t.up[3 * el + 1] = ro.up_vec[1]; t.up[3 * el + 2] = ro.up_vec[2];
+        t.head[3 * el] = ro.heading_vec[0]; t.head[3 * el + 1] = ro.heading_vec[1]; t.head[3 * el + 2] = ro.heading_vec[2];
+        t.to[el] = r.timed;
     }
     fence_async_smem();
     __syncthreads();
     // one bulk-async (TMA) store per output tensor.  The stores are dealt to the FIRST THREAD of each warp at compile time
     // (`threadIdx.x == 32 w` branches, each a single-thread region the compiler keeps on the uniform datapath): their issue
     // -- address arithmetic + UBLKCP each -- runs in parallel instead of as one thread's serial tail
+    static_assert(EPB % 16 == 0, "bulk copies move multiples of 16 bytes: the timeout tile is EPB bytes");
+    const size_t e0 = (size_t)env0;
     {
-        const size_t e0 = (size_t)env0;
         float *const g_act_out = (float *)B.p[B2G_T_ACTIONS];
         constexpr int NW = BLOCK / 32;
         auto issue = [&](int w) {
             int k = 0;
 #define B2G_ST(COND, DST, SRC, BYTES) do { if ((k++ % NW) == w) { if (COND) bulk_s2g(DST, SRC, BYTES); } } while (0)
-            B2G_ST(true, g_obs + e0 * O, t_obs, (uint32_t)(EPB * O * 4));
-            B2G_ST(g_obsc != nullptr, g_obsc + e0 * O, t_obsc, (uint32_t)(EPB * O * 4));
+            B2G_ST(true, g_obs + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
+            B2G_ST(g_obsc != nullptr, g_obsc + e0 * O, t.obsc, (uint32_t)(EPB * O * 4));
             B2G_ST(true, (float *)B.p[B2G_T_ROOT_STATE] + e0 * 13, s_root, EPB * 13 * 4);
             B2G_ST(true, (float *)B.p[B2G_T_DOF_STATE] + e0 * nd * 2, s_dof, (uint32_t)(EPB * nd * 8));
             B2G_ST(g_act_out != nullptr, g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
             B2G_ST(stage_out && g_sens && nsens6, g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
-            B2G_ST(true, (float *)B.p[B2G_T_REW] + e0, t_rew, EPB * 4);
-            B2G_ST(true, pot_b + e0, t_pot, EPB * 4);
-            B2G_ST(true, ppot_b + e0, t_ppot, EPB * 4);
-            B2G_ST(B.p[B2G_T_UP_VEC] != nullptr, (float *)B.p[B2G_T_UP_VEC] + 3 * e0, t_up, EPB * 12);
-            B2G_ST(B.p[B2G_T_HEADING_VEC] != nullptr, (float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t_head, EPB * 12);
-            B2G_ST(true, reset_b + e0, t_reset, EPB * 8);
-            B2G_ST(true, progress_b + e0, t_prog, EPB * 8);
-            if (EPB % 16 == 0) B2G_ST(B.p[B2G_T_TIMEOUT] != nullptr, (uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t_to, EPB);   // bulk copies move multiples of 16 bytes
+            B2G_ST(true, (float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
+            B2G_ST(true, pot_b + e0, t.pot, EPB * 4);
+            B2G_ST(true, ppot_b + e0, t.ppot, EPB * 4);
+            B2G_ST(B.p[B2G_T_UP_VEC] != nullptr, (float *)B.p[B2G_T_UP_VEC] + 3 * e0, t.up, EPB * 12);
+            B2G_ST(B.p[B2G_T_HEADING_VEC] != nullptr, (float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t.head, EPB * 12);
+            B2G_ST(true, reset_b + e0, t.reset, EPB * 8);
+            B2G_ST(true, progress_b + e0, t.prog, EPB * 8);
+            B2G_ST(B.p[B2G_T_TIMEOUT] != nullptr, (uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
 #undef B2G_ST
             bulk_commit_wait();
         };
-        if (EPB % 16 != 0 && B.p[B2G_T_TIMEOUT] && threadIdx.x < EPB) ((uint8_t *)B.p[B2G_T_TIMEOUT])[e0 + threadIdx.x] = t_to[threadIdx.x];
         if (threadIdx.x == 0) issue(0);
         else if (NW > 1 && threadIdx.x == 32) issue(1);
         else if (NW > 2 && threadIdx.x == 64) issue(2);
         else if (NW > 3 && threadIdx.x == 96) issue(3);
     }
-    if (HOSTIO) {                  // host copies of what VecTask.step returns (vec_task.py:402-408), straight over PCIe
-        const size_t e0 = (size_t)env0;
-        auto copy16 = [&](void *dst, const void *src, int bytes) {
-            float4 *d = reinterpret_cast<float4 *>(dst); const float4 *sp = reinterpret_cast<const float4 *>(src);
-            for (int i = threadIdx.x; i < bytes / 16; i += BLOCK) d[i] = sp[i];
-        };
-        if (ta.h_obs) copy16(ta.h_obs + e0 * O, g_obsc ? t_obsc : t_obs, EPB * O * 4);
-        if (ta.h_rew) copy16(ta.h_rew + e0, t_rew, EPB * 4);
-        if (ta.h_reset) copy16(ta.h_reset + e0, t_reset, EPB * 8);
-        if (ta.h_timeout) {
-            if (EPB % 16 == 0) copy16(ta.h_timeout + e0, t_to, EPB);
-            else if (threadIdx.x < EPB) ta.h_timeout[e0 + threadIdx.x] = t_to[threadIdx.x];
-        }
-    }
+    if (HOSTIO) loco_copy_to_host<BLOCK>(ta, t, e0, EPB, O, g_obsc != nullptr);
 }
 
 

@@ -25,6 +25,36 @@ struct RollArgs {
     int io_f4, model_f4, stage_f4;     // float4 offsets inside dynamic shared memory
 };
 
+// output staging of the rollout, epb envs per block.  Per step (never aliases the sweep scratch):
+// obs | rew | reset(i64) | timeout(u8).  Last step only, the remaining state tensors in the (then dead) sweep scratch:
+// obs (unclipped, when a separate clipped tensor exists) | pot | ppot | up(3) | head(3) | progress(i64)
+struct RollStage {
+    float *obs, *rew;
+    long long *reset;
+    uint8_t *to;
+};
+struct RollLast {
+    float *obs, *pot, *ppot, *up, *head;
+    long long *prog;
+};
+__device__ __forceinline__ RollStage roll_stage(float *base, int epb, int O) {
+    RollStage t;
+    t.obs = base;
+    t.rew = t.obs + epb * O;
+    t.reset = reinterpret_cast<long long *>(t.rew + epb);
+    t.to = reinterpret_cast<uint8_t *>(t.reset + epb);
+    return t;
+}
+__device__ __forceinline__ RollLast roll_last(float *base, int epb, int O) {
+    RollLast l;
+    l.obs = base;
+    l.pot = l.obs + epb * O; l.ppot = l.pot + epb; l.up = l.ppot + epb; l.head = l.up + 3 * epb;
+    l.prog = reinterpret_cast<long long *>(l.head + 3 * epb);
+    return l;
+}
+__host__ __device__ inline size_t roll_stage_bytes(int epb, int O) { return (size_t)epb * (O * 4 + 4 + 8 + 1); }
+__host__ __device__ inline size_t roll_last_bytes(int epb, int O) { return (size_t)epb * (O * 4 + 4 * 2 + 12 * 2 + 8); }
+
 template <int NS, int SP>
 __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__restrict__ gqm, Buffers B, const __grid_constant__ b2g_task_params P,
                                                               int N, int substeps, const __grid_constant__ RollArgs ra) {
@@ -41,15 +71,8 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
     float *const s_dof = s_root + EPB * 13;
     float *const s_actb[2] = {s_dof + EPB * nd * 2, s_dof + EPB * nd * 2 + EPB * nd};
     float *const s_sens = s_actb[1] + EPB * nd;
-    // per-step output staging (never aliases the sweep scratch): obs | rew | reset(i64) | timeout(u8)
-    float *const t_obs = stage;
-    float *const t_rew = t_obs + EPB * O;
-    long long *const t_reset = reinterpret_cast<long long *>(t_rew + EPB);
-    uint8_t *const t_to = reinterpret_cast<uint8_t *>(t_reset + EPB);
-    // last-step staging of the remaining state tensors, in the (then dead) sweep scratch
-    float *const l_obs = reinterpret_cast<float *>(park);
-    float *const l_pot = l_obs + EPB * O, *const l_ppot = l_pot + EPB, *const l_up = l_ppot + EPB, *const l_head = l_up + 3 * EPB;
-    long long *const l_prog = reinterpret_cast<long long *>(l_head + 3 * EPB);
+    const RollStage t = roll_stage(stage, EPB, O);
+    const RollLast l = roll_last(reinterpret_cast<float *>(park), EPB, O);
     long long *const progress_b = (long long *)B.p[B2G_T_PROGRESS];
     long long *const reset_b = (long long *)B.p[B2G_T_RESET];
     float *const pot_b = (float *)B.p[B2G_T_POTENTIALS], *const ppot_b = (float *)B.p[B2G_T_PREV_POTENTIALS];
@@ -137,111 +160,38 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
         if (do_reset) {                                       // reset_idx, ant.py:252-279
 #pragma unroll
             for (int s = 0; s < NS; s++) {
-                const int d = dofi[s];
-                const float up = reset_uniform(P.seed, gid, count, d);
-                const float uv = reset_uniform(P.seed, gid, count, nd + d);
-                const float pos = (P.reset_pos_noise - (-P.reset_pos_noise)) * up + (-P.reset_pos_noise);
-                L.q[s] = fmaxf(fminf(P.initial_dof_pos[d] + pos, P.dof_limits_upper[d]), P.dof_limits_lower[d]);
-                L.qd[s] = (P.reset_vel_noise - (-P.reset_vel_noise)) * uv + (-P.reset_vel_noise);
+                const float2 qv = loco_reset_dof(P, gid, count, dofi[s], nd);
+                L.q[s] = qv.x; L.qd[s] = qv.y;
             }
-            const float *ir = (const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e;
-            load_root(ir, rs);
-            potentials = t_potential(P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], P.dt);
+            potentials = loco_reset_root(P, B, e, rs);
             progress = 0;
             count += 1;
         }
         // the previous step's output stores must have read their staging tiles before these are rewritten
         if ((threadIdx.x & 31) == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         __syncthreads();
-        float *const obs = t_obs + (size_t)el * O;            // per-step output tile: the observation step() returns
-        float *const obs_raw = l_obs + (size_t)el * O;        // last step only, when a separate unclipped tensor exists
-        const float to_t[3] = {P.target[0] - rs.rp[0], P.target[1] - rs.rp[1], 0.f};
+        float *const obs = t.obs + (size_t)el * O;            // per-step output tile: the observation step() returns
+        float *const obs_raw = l.obs + (size_t)el * O;        // last step only, when a separate unclipped tensor exists
         const float prev_potentials = potentials;
-        potentials = t_potential(to_t[0], to_t[1], P.dt);
-        const float isr[4] = {-0.f, -0.f, -0.f, 1.f};
-        float tq[4]; t_quat_mul(rs.rq, isr, tq);
-        float ang_mine;
-        {
-            const float qx = tq[0], qy = tq[1], qz = tq[2], qw = tq[3];
-            const float ay = (lane == 1) ? 2.0f * (qw * qx + qy * qz) : (lane == 2) ? P.target[2] - rs.rp[2] : 2.0f * (qw * qz + qx * qy);
-            const float ax = (lane == 1) ? qw * qw - qx * qx - qy * qy + qz * qz : (lane == 2) ? P.target[0] - rs.rp[0] : qw * qw + qx * qx - qy * qy - qz * qz;
-            const float a = atan2f(ay, ax);
-            ang_mine = (lane != 2 && a < 0.f) ? a + 6.2831855f : a;
-        }
-        const float roll = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 1);
-        const float walk = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28) | 2);
-        const float yaw = __shfl_sync(0xffffffffu, ang_mine, (threadIdx.x & 28));
-        auto put = [&](int idx, float v) {
-            obs[idx] = clip_sep ? fminf(fmaxf(v, -clipo), clipo) : v;
-            if (last && clip_sep) obs_raw[idx] = v;
-        };
-        float up_proj = 0.f, heading_proj = 0.f;
-        float up_vec[3], heading_vec[3];
-        if (lane == 0) {
-            const float nrm = fmaxf(sqrtf(to_t[0] * to_t[0] + to_t[1] * to_t[1] + 0.f), 1e-9f);
-            const float td[3] = {to_t[0] / nrm, to_t[1] / nrm, 0.f / nrm};
-            const float b0[3] = {1.f, 0.f, 0.f}, b1[3] = {0.f, 0.f, 1.f};
-            t_quat_rotate(tq, b1, up_vec, 1.f);
-            t_quat_rotate(tq, b0, heading_vec, 1.f);
-            up_proj = up_vec[2];
-            heading_proj = (heading_vec[0] * td[0] + heading_vec[1] * td[1]) + heading_vec[2] * td[2];
-            float vloc[3], wloc[3];
-            t_quat_rotate(tq, rs.rv, vloc, -1.f);
-            t_quat_rotate(tq, rs.rw, wloc, -1.f);
-            put(0, rs.rp[2]);
-            put(1, vloc[0]); put(2, vloc[1]); put(3, vloc[2]);
-            put(4, wloc[0]); put(5, wloc[1]); put(6, wloc[2]);
-            put(7, yaw); put(8, roll); put(9, walk - yaw); put(10, up_proj); put(11, heading_proj);
-        }
-        const int o_pos = 12, o_vel = 12 + nd, o_sens = 12 + 2 * nd, o_act = o_sens + nsens6;
-        float actions_cost = 0.f, electricity = 0.f, at_limit = 0.f;
-#pragma unroll
-        for (int s = 0; s < NS; s++) {
-            const int d = dofi[s];
-            const float a = a_cl[s];
-            const float ps = t_unscale(L.q[s], P.dof_limits_lower[d], P.dof_limits_upper[d]);
-            const float vs = L.qd[s] * P.dof_vel_scale;
-            put(o_pos + d, ps); put(o_vel + d, vs); put(o_act + d, a);
-            if (sens[s] >= 0) {
-                float sv[6];
-                if (stage_out) {
-                    const float *sp_ = s_sens + nsens6 * el + 6 * sens[s];
-#pragma unroll
-                    for (int c = 0; c < 6; c++) sv[c] = sp_[c];
-                } else {
-#pragma unroll
-                    for (int c = 0; c < 6; c++) sv[c] = g_sens ? g_sens[(size_t)e * nsens6 + 6 * sens[s] + c] : 0.f;
-                }
-                if (stage_out || g_sens) {
-#pragma unroll
-                    for (int c = 0; c < 6; c++) put(o_sens + 6 * sens[s] + c, sv[c] * P.contact_force_scale);
-                }
-            }
-            actions_cost += a * a;
-            at_limit += (ps > 0.99f) ? 1.f : 0.f;
-            electricity += fabsf(a * vs);
-        }
-        actions_cost = lane_sum<4>(actions_cost);
-        electricity = lane_sum<4>(electricity);
-        at_limit = lane_sum<4>(at_limit);
+        potentials = loco_potential(P, rs.rp);
+        AntRootObs ro;
+        LocoCosts cost = ant_obs<NS>(P, rs, L.q, L.qd, dofi, sens, a_cl, qm, lane, s_sens, g_sens, e, el, nsens6, stage_out, ro,
+                                     [&](int idx, float v) {
+                                         obs[idx] = clip_sep ? fminf(fmaxf(v, -clipo), clipo) : v;
+                                         if (last && clip_sep) obs_raw[idx] = v;
+                                     });
+        cost.sum_lanes<4>();
         // reset / time-out depend on the height and the step count only: every lane of the env knows them (the flag drives
         // the NEXT step's reset_idx on all four lanes)
-        const bool timed = (float)progress >= P.max_episode_length - 1.f;
-        const bool died = rs.rp[2] < P.termination_height;
-        do_reset = died || timed;
+        const LocoReward r = loco_reward(P, ro.up_proj, ro.heading_proj, potentials, prev_potentials, cost, rs.rp[2], progress, false);
+        do_reset = r.died || r.timed;
         if (lane == 0) {
-            const float heading_reward = (heading_proj > 0.8f) ? P.heading_weight : P.heading_weight * heading_proj / 0.8f;
-            const float up_reward = (up_proj > 0.93f) ? P.up_weight : 0.f;
-            const float progress_reward = potentials - prev_potentials;
-            float total_r = progress_reward + P.alive_reward + up_reward + heading_reward - P.actions_cost_scale * actions_cost -
-                            P.energy_cost_scale * electricity - at_limit * P.joints_at_limit_cost_scale;
-            if (died) total_r = P.death_cost;
-            t_rew[el] = total_r; t_reset[el] = do_reset ? 1 : 0;
-            t_to[el] = (uint8_t)(timed && do_reset);                                                      // vec_task.py:394
+            t.rew[el] = r.rew; t.reset[el] = do_reset ? 1 : 0;
+            t.to[el] = r.timed;                                                                             // vec_task.py:394
             if (last) {
-                l_pot[el] = potentials; l_ppot[el] = prev_potentials; l_prog[el] = progress;
-                l_up[3 * el] = up_vec[0]; l_up[3 * el + 1] = up_vec[1]; l_up[3 * el + 2] = up_vec[2];
-                l_head[3 * el] = heading_vec[0]; l_head[3 * el + 1] = heading_vec[1]; l_head[3 * el + 2] = heading_vec[2];
+                l.pot[el] = potentials; l.ppot[el] = prev_potentials; l.prog[el] = progress;
+                l.up[3 * el] = ro.up_vec[0]; l.up[3 * el + 1] = ro.up_vec[1]; l.up[3 * el + 2] = ro.up_vec[2];
+                l.head[3 * el] = ro.heading_vec[0]; l.head[3 * el + 1] = ro.heading_vec[1]; l.head[3 * el + 2] = ro.heading_vec[2];
                 if (count != count0) rc[e] = (int)count;
             }
         }
@@ -255,30 +205,30 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
         {
             const size_t e0 = (size_t)env0, kN = (size_t)kk * N + e0;
             if (threadIdx.x == 0) {
-                bulk_s2g(ra.obs_out + kN * O, t_obs, (uint32_t)(EPB * O * 4));
-                bulk_s2g(ra.rew_out + kN, t_rew, EPB * 4);
+                bulk_s2g(ra.obs_out + kN * O, t.obs, (uint32_t)(EPB * O * 4));
+                bulk_s2g(ra.rew_out + kN, t.rew, EPB * 4);
                 if (last) {
                     float *const g_act_out = (float *)B.p[B2G_T_ACTIONS];
-                    bulk_s2g(g_obs + e0 * O, clip_sep ? l_obs : t_obs, (uint32_t)(EPB * O * 4));
-                    if (clip_sep) bulk_s2g(g_obsc + e0 * O, t_obs, (uint32_t)(EPB * O * 4));
+                    bulk_s2g(g_obs + e0 * O, clip_sep ? l.obs : t.obs, (uint32_t)(EPB * O * 4));
+                    if (clip_sep) bulk_s2g(g_obsc + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
                     bulk_s2g((float *)B.p[B2G_T_ROOT_STATE] + e0 * 13, s_root, EPB * 13 * 4);
                     bulk_s2g((float *)B.p[B2G_T_DOF_STATE] + e0 * nd * 2, s_dof, (uint32_t)(EPB * nd * 8));
                     if (g_act_out) bulk_s2g(g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
                 }
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             } else if (threadIdx.x == 32) {
-                bulk_s2g(ra.reset_out + kN, t_reset, EPB * 8);
-                if (ra.timeout_out) bulk_s2g(ra.timeout_out + kN, t_to, EPB);
+                bulk_s2g(ra.reset_out + kN, t.reset, EPB * 8);
+                if (ra.timeout_out) bulk_s2g(ra.timeout_out + kN, t.to, EPB);
                 if (last) {
                     if (stage_out && g_sens && nsens6) bulk_s2g(g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
-                    bulk_s2g((float *)B.p[B2G_T_REW] + e0, t_rew, EPB * 4);
-                    bulk_s2g(pot_b + e0, l_pot, EPB * 4);
-                    bulk_s2g(ppot_b + e0, l_ppot, EPB * 4);
-                    if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, l_up, EPB * 12);
-                    if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, l_head, EPB * 12);
-                    bulk_s2g(reset_b + e0, t_reset, EPB * 8);
-                    bulk_s2g(progress_b + e0, l_prog, EPB * 8);
-                    if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t_to, EPB);
+                    bulk_s2g((float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
+                    bulk_s2g(pot_b + e0, l.pot, EPB * 4);
+                    bulk_s2g(ppot_b + e0, l.ppot, EPB * 4);
+                    if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, l.up, EPB * 12);
+                    if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, l.head, EPB * 12);
+                    bulk_s2g(reset_b + e0, t.reset, EPB * 8);
+                    bulk_s2g(progress_b + e0, l.prog, EPB * 8);
+                    if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
                 }
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }

@@ -24,16 +24,11 @@ __global__ void __launch_bounds__(128) loco_reset_kernel(Buffers B, const __grid
         for (int s = 0; s < 2; s++)
             dof[s] = make_float2(0.2f * (reset_uniform(P.seed, gid, count, s) - 0.5f), 0.5f * (reset_uniform(P.seed, gid, count, 2 + s) - 0.5f));
     } else {
-        for (int d = 0; d < nd; d++) {
-            const float up = reset_uniform(P.seed, gid, count, d), uv = reset_uniform(P.seed, gid, count, nd + d);
-            const float pos = (P.reset_pos_noise - (-P.reset_pos_noise)) * up + (-P.reset_pos_noise);
-            dof[d] = make_float2(fmaxf(fminf(P.initial_dof_pos[d] + pos, P.dof_limits_upper[d]), P.dof_limits_lower[d]),
-                                 (P.reset_vel_noise - (-P.reset_vel_noise)) * uv + (-P.reset_vel_noise));
-        }
+        for (int d = 0; d < nd; d++) dof[d] = loco_reset_dof(P, gid, count, d, nd);
         const float *ir = (const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e;
         float *r = (float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e;
         for (int c = 0; c < 13; c++) r[c] = ir[c];
-        const float pot = t_potential(P.target[0] - ir[0], P.target[1] - ir[1], P.dt);
+        const float pot = loco_potential(P, ir);
         ((float *)B.p[B2G_T_POTENTIALS])[e] = pot;                       // prev_potentials = potentials = -|to_target| / dt (:273-276)
         ((float *)B.p[B2G_T_PREV_POTENTIALS])[e] = pot;
     }

@@ -5,8 +5,7 @@
 // by the reference's own functions (tests/golden) at 1e-6, and `potentials` bit-exactly, because
 // progress_reward = potentials - prev_potentials (tasks/ant.py:359) differences two ~6e4 numbers.
 #pragma once
-#include "b2g_device.cuh"
-#include "../../include/b200gym.h"
+#include "b2g_common.cuh"
 
 namespace b2g {
 
@@ -87,6 +86,11 @@ __device__ __forceinline__ float reset_uniform(uint64_t seed, uint32_t env, uint
 }
 
 // ------------------------------------------------------------------ locomotion (Ant / Humanoid)
+// potentials from a root position (ant.py:273-275, 387-391)
+__device__ __forceinline__ float loco_potential(const b2g_task_params &P, const float rp[3]) {
+    return t_potential(P.target[0] - rp[0], P.target[1] - rp[1], P.dt);
+}
+
 // Root-derived part of compute_ant_observations (ant.py:374-408) /
 // compute_humanoid_observations (humanoid.py:378-413): fills o[0..11] and the per-env state.
 struct LocoRootObs {
@@ -96,7 +100,7 @@ struct LocoRootObs {
 __device__ __forceinline__ void loco_root_obs(const b2g_task_params &P, const float rp[3], const float rq[4],
                                               const float rv[3], const float rw[3], bool humanoid, LocoRootObs &r) {
     const float to_t[3] = {P.target[0] - rp[0], P.target[1] - rp[1], 0.f};
-    r.potentials = t_potential(to_t[0], to_t[1], P.dt);
+    r.potentials = loco_potential(P, rp);
     // compute_heading_and_up, torch_jit_utils.py:247-262 (inv_start_rot = identity conj, ant.py:106)
     const float nrm = fmaxf(sqrtf(to_t[0] * to_t[0] + to_t[1] * to_t[1] + 0.f), 1e-9f);
     const float td[3] = {to_t[0] / nrm, to_t[1] / nrm, 0.f / nrm};
@@ -124,6 +128,102 @@ __device__ __forceinline__ void loco_root_obs(const b2g_task_params &P, const fl
 
 // unscale, torch_jit_utils.py:238-239
 __device__ __forceinline__ float t_unscale(float x, float lo, float hi) { return (2.0f * x - hi - lo) / (hi - lo); }
+
+// reset_idx (ant.py:252-279, humanoid.py:253-279): DOF d of env `gid`'s reset number `count` -- the initial position plus
+// uniform noise, clamped to the limits, and a uniform velocity
+__device__ __forceinline__ float2 loco_reset_dof(const b2g_task_params &P, uint32_t gid, uint32_t count, int d, int nd) {
+    const float up = reset_uniform(P.seed, gid, count, d);
+    const float uv = reset_uniform(P.seed, gid, count, nd + d);
+    const float pos = (P.reset_pos_noise - (-P.reset_pos_noise)) * up + (-P.reset_pos_noise);
+    return make_float2(fmaxf(fminf(P.initial_dof_pos[d] + pos, P.dof_limits_upper[d]), P.dof_limits_lower[d]),
+                       (P.reset_vel_noise - (-P.reset_vel_noise)) * uv + (-P.reset_vel_noise));
+}
+
+// reset_idx's root: the initial root state; returns the potential that prev_potentials and potentials are both reset to
+__device__ __forceinline__ float loco_reset_root(const b2g_task_params &P, const Buffers &B, int e, RootState &rs) {
+    load_root((const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e, rs);
+    return loco_potential(P, rs.rp);
+}
+
+// the per-DOF sums of compute_ant_reward (ant.py:353-355) / compute_humanoid_reward (humanoid.py:352-359), from the clamped
+// action a and the observed ps (unscaled position) and vs (scaled velocity)
+struct LocoCosts {
+    float actions = 0.f, electricity = 0.f, at_limit = 0.f;
+    __device__ __forceinline__ void add(const b2g_task_params &P, int d, float a, float ps, float vs, bool humanoid) {
+        actions += a * a;
+        if (humanoid) {
+            const float ratio = P.motor_efforts[d] / P.max_motor_effort;
+            const float scaled = P.joints_at_limit_cost_scale * (fabsf(ps) - 0.98f) / 0.02f;
+            at_limit += (fabsf(ps) > 0.98f) ? scaled * ratio : 0.f;
+            electricity += fabsf(a * vs) * ratio;
+        } else {
+            at_limit += (ps > 0.99f) ? 1.f : 0.f;
+            electricity += fabsf(a * vs);
+        }
+    }
+    template <int L> __device__ __forceinline__ void sum_lanes() {
+        actions = lane_sum<L>(actions);
+        electricity = lane_sum<L>(electricity);
+        at_limit = lane_sum<L>(at_limit);
+    }
+};
+
+// the rest of compute_ant_reward (ant.py:326-371) / compute_humanoid_reward (humanoid.py:324-375): the reward and the two
+// reasons to reset -- the torso fell below termination_height (the reward is then death_cost) or the episode ran out.
+// reset_buf was cleared by reset_idx or was already 0, so reset = died || timed, and time_out = timed (vec_task.py:394).
+struct LocoReward {
+    float rew;
+    bool died, timed;
+};
+__device__ __forceinline__ LocoReward loco_reward(const b2g_task_params &P, float up_proj, float heading_proj, float potentials,
+                                                  float prev_potentials, const LocoCosts &c, float height, long long progress,
+                                                  bool humanoid) {
+    const float heading_reward = (heading_proj > 0.8f) ? P.heading_weight : P.heading_weight * heading_proj / 0.8f;
+    const float up_reward = (up_proj > 0.93f) ? P.up_weight : 0.f;
+    const float progress_reward = potentials - prev_potentials;
+    LocoReward r;
+    r.rew = progress_reward + P.alive_reward + up_reward + heading_reward - P.actions_cost_scale * c.actions -
+            P.energy_cost_scale * c.electricity - (humanoid ? c.at_limit : c.at_limit * P.joints_at_limit_cost_scale);
+    r.died = height < P.termination_height;
+    if (r.died) r.rew = P.death_cost;
+    r.timed = (float)progress >= P.max_episode_length - 1.f;
+    return r;
+}
+
+// output staging of the fused Ant / Humanoid steps, epb envs per block (floats unless noted):
+// obs | obs_clipped (only when it is a separate tensor) | rew | pot | ppot | up(3) | head(3) | reset(i64) | progress(i64) | timeout(u8)
+struct LocoStage {
+    float *obs, *obsc, *rew, *pot, *ppot, *up, *head;
+    long long *reset, *prog;
+    uint8_t *to;
+};
+__device__ __forceinline__ LocoStage loco_stage(float *base, int epb, int O, bool clip_sep) {
+    LocoStage t;
+    t.obs = base;
+    t.obsc = t.obs + epb * O;
+    t.rew = t.obsc + (clip_sep ? epb * O : 0);
+    t.pot = t.rew + epb; t.ppot = t.pot + epb; t.up = t.ppot + epb; t.head = t.up + 3 * epb;
+    t.reset = reinterpret_cast<long long *>(t.head + 3 * epb); t.prog = t.reset + epb;
+    t.to = reinterpret_cast<uint8_t *>(t.prog + epb);
+    return t;
+}
+__host__ __device__ inline size_t loco_stage_bytes(int epb, int O, bool clip_sep) {
+    return (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1);
+}
+
+// b2g_task_step_host: what VecTask.step returns (vec_task.py:402-408), from the staging tiles straight to the pinned host
+// buffers over PCIe as coalesced 16-byte stores.  Whole tiles only (epb % 16 == 0): every copy is a multiple of 16 bytes.
+template <int BLOCK>
+__device__ __forceinline__ void loco_copy_to_host(const TileArgs &ta, const LocoStage &t, size_t e0, int epb, int O, bool clip_sep) {
+    auto copy16 = [&](void *dst, const void *src, int bytes) {
+        float4 *d = reinterpret_cast<float4 *>(dst); const float4 *sp = reinterpret_cast<const float4 *>(src);
+        for (int i = threadIdx.x; i < bytes / 16; i += BLOCK) d[i] = sp[i];
+    };
+    if (ta.h_obs) copy16(ta.h_obs + e0 * O, clip_sep ? t.obsc : t.obs, epb * O * 4);
+    if (ta.h_rew) copy16(ta.h_rew + e0, t.rew, epb * 4);
+    if (ta.h_reset) copy16(ta.h_reset + e0, t.reset, epb * 8);
+    if (ta.h_timeout) copy16(ta.h_timeout + e0, t.to, epb);
+}
 
 // compute_cartpole_reward, cartpole.py:180-196
 __device__ __forceinline__ void cartpole_reward(float pole_angle, float pole_vel, float cart_vel, float cart_pos,
