@@ -67,8 +67,9 @@ typedef struct {
      * that are not joint neighbours collide with each other.  self_pairs: ncp x ncp bytes, 1 = the ordered pair may collide
      * (NULL / self_collide 0 = off).  Same contact law as the ground contact; self_kn, self_cn are DIMENSIONLESS: per pair
      * kn = self_kn m_red / h^2, cn = self_cn m_red / h with the reduced mass of the two links (stability of the half-explicit
-     * coupling; 0.5 / 0.5 is what the importer sets); generic sub-step only
-     * (ncp <= 64, no second actor); a four-chain model with self_collide set runs on the generic path. */
+     * coupling; 0.5 / 0.5 is what the importer sets); ncp <= 64, no second actor.  A four-chain model with chain length 3
+     * (ANYmal) keeps the four-chain kernels, which carry the contact when no candidate pair lies within one leg; every other
+     * self-colliding model, the chain-length-2 one (Ant) included, runs on the generic sub-step. */
     int32_t self_collide, pad_self;
     const uint8_t *self_pairs;
     float self_kn, self_cn, self_mu, pad_self2;

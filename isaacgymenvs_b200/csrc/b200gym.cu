@@ -758,17 +758,22 @@ static int launch(b2g_sim *s, void (*kernel)(P...), int grid, int block, size_t 
 // ShadowHand, AnymalTerrain, (Cartpole), quad locomotion, locomotion, (rollout).
 static constexpr int key(int lanes, int block) { return (lanes << 8) | block; }
 
-// gym.simulate() on the quad sub-step: (chain length, height field, specialisation); 128 threads, one env per 4
+// gym.simulate() on the quad sub-step: (chain length, height field, specialisation, link-link contact); 128 threads, one
+// env per 4.  A self-colliding model is packed for chain length 3 in the general layout (quad_build)
 constexpr int QUAD_SIM_BLOCK = 128;
 using QuadSimKernel = void (*)(const float4 *, const int16_t *, Buffers, int, int);
-static QuadSimKernel quad_simulate_kernel_for(int ns, bool hf, int spec) {
+static QuadSimKernel quad_simulate_kernel_for(int ns, bool hf, int spec, bool self) {
     constexpr int B = QUAD_SIM_BLOCK;
     const bool sp3 = spec == 3;
-    if (ns == 2 && !hf) return sp3 ? quad_simulate_kernel<2, false, 3, B> : quad_simulate_kernel<2, false, 0, B>;
-    if (ns == 2) return sp3 ? quad_simulate_kernel<2, true, 3, B> : quad_simulate_kernel<2, true, 0, B>;
-    if (ns == 3 && !hf) return sp3 ? quad_simulate_kernel<3, false, 3, B> : quad_simulate_kernel<3, false, 0, B>;
-    if (ns == 3) return sp3 ? quad_simulate_kernel<3, true, 3, B> : quad_simulate_kernel<3, true, 0, B>;
-    return nullptr;
+    if (!self) {
+        if (ns == 2 && !hf) return sp3 ? quad_simulate_kernel<2, false, 3, B> : quad_simulate_kernel<2, false, 0, B>;
+        if (ns == 2) return sp3 ? quad_simulate_kernel<2, true, 3, B> : quad_simulate_kernel<2, true, 0, B>;
+        if (ns == 3 && !hf) return sp3 ? quad_simulate_kernel<3, false, 3, B> : quad_simulate_kernel<3, false, 0, B>;
+        if (ns == 3) return sp3 ? quad_simulate_kernel<3, true, 3, B> : quad_simulate_kernel<3, true, 0, B>;
+        return nullptr;
+    }
+    if (ns != 3 || spec != 0) return nullptr;
+    return hf ? quad_simulate_kernel<3, true, 0, B, true> : quad_simulate_kernel<3, false, 0, B, true>;
 }
 
 // gym.simulate() on the generic Stepper: (lanes, CTA size, height field, free object, self-collision, per-env physical
@@ -833,8 +838,9 @@ extern "C" int b2g_simulate(b2g_sim *s, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const int N = s->num_envs;
     if (s->quad_ns) {
-        const size_t dyn = ((size_t)quad_park_f4(s->quad_ns) * QUAD_SIM_BLOCK + quad_model_f4(s->quad_ns)) * sizeof(float4);
-        return launch(s, quad_simulate_kernel_for(s->quad_ns, s->d_hf != nullptr, s->quad_spec), (N * 4 + QUAD_SIM_BLOCK - 1) / QUAD_SIM_BLOCK,
+        const bool self = s->hm.self_on != 0;
+        const size_t dyn = ((size_t)quad_park_f4(s->quad_ns, self) * QUAD_SIM_BLOCK + quad_model_f4(s->quad_ns, self)) * sizeof(float4);
+        return launch(s, quad_simulate_kernel_for(s->quad_ns, s->d_hf != nullptr, s->quad_spec, self), (N * 4 + QUAD_SIM_BLOCK - 1) / QUAD_SIM_BLOCK,
                       QUAD_SIM_BLOCK, dyn, st, SMEM, s->d_qm, s->d_hf, s->buf, N, s->hm.substeps);
     }
     const int blk = s->block, grid = (N * s->lanes + blk - 1) / blk;
@@ -999,15 +1005,19 @@ static int hand_step(b2g_sim *s, const float *actions, void *stream) {
 }
 
 // AnymalTerrain physics (the first of its two kernels): the quad sub-step when the model is on the quad path (on a height
-// field with or without per-env physical parameters), else the generic Stepper; plane or height field.  128 threads.
+// field with or without per-env physical parameters; with link-link contact when the model self-collides), else the
+// generic Stepper; plane or height field.  128 threads.
 static int launch_anymal_physics(b2g_sim *s, const b2g_anymal_params &P, const float *actions, int N, int grid, cudaStream_t st) {
-    const bool hf = s->d_hf != nullptr;
+    const bool hf = s->d_hf != nullptr, self = s->hm.self_on != 0;
     if (s->quad_ns == 3) {
         const bool dr = s->buf.p[B2G_T_ENV_MASS_SCALE] || s->buf.p[B2G_T_ENV_DOF_PROPS];
-        const auto k = hf ? (dr ? quad_anymal_physics_kernel<true, 128, true> : quad_anymal_physics_kernel<true, 128, false>) : quad_anymal_physics_kernel<false, 128>;
-        const size_t dyn = ((size_t)quad_park_f4(3) * 128 + quad_model_f4(3)) * sizeof(float4);
+        auto k = hf ? (dr ? quad_anymal_physics_kernel<true, 128, true> : quad_anymal_physics_kernel<true, 128, false>) : quad_anymal_physics_kernel<false, 128>;
+        if (self) k = hf ? quad_anymal_physics_kernel<true, 128, true, true> : quad_anymal_physics_kernel<false, 128, true, true>;
+        const size_t dyn = ((size_t)quad_park_f4(3, self) * 128 + quad_model_f4(3, self)) * sizeof(float4);
         return launch(s, k, grid, 128, dyn, st, SMEM, s->d_qm, s->d_hf, s->buf, P, actions, N, s->hm.substeps, s->step_counter);
     }
+    // the generic AnymalTerrain kernel has no link-link contact: never drop it silently
+    if (self) return fail(B2G_E_UNSUPPORTED, "b2g_task_step(AnymalTerrain): link-link contact needs the four-chain kernels (unset B2G_NO_QUAD)");
     const auto k = hf ? anymal_physics_kernel<4, true, 128> : anymal_physics_kernel<4, false, 128>;
     return launch(s, k, grid, 128, s->dyn_smem, st, SMEM, s->dm, s->d_hf, s->buf, P, actions, N, s->step_counter);
 }

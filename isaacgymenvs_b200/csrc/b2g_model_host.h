@@ -298,7 +298,7 @@ static inline int build_sim_model(const b2g_model *m, const b2g_model_ext *ext, 
     // the specialised path of "four hinge chains on a free base" (Ant, ANYmal): b2g_quad.cuh
     out.quad_ns = out.quad_spec = 0;
     out.qm.clear();
-    if (!no_quad && !ext && !h.self_on && !single_lane) {
+    if (!no_quad && !ext && !single_lane) {                              // a self-colliding model: ANYmal-class only (quad_build)
         int leg_link[12];
         out.quad_ns = quad_build(m, sp, out.qm, leg_link, &out.quad_spec);
     }

@@ -31,13 +31,18 @@ namespace b2g {
 // link block k: 0..6 M0 M1 M2 axp[0] | 7: axp[1] axp[2] lpos[0] lpos[1] | 8: lpos[2] com xyz | 9: Ic xx yy zz xy
 //  10: Ic xz yz, mass, dg0 | 11: damping stiffness lower upper | 12: effort limit_k limit_d limit_dg | 13,14: spheres (pos, radius; radius<0 unused)
 //  15: mu0 mu1 sbpos.x sbpos.y | 16: sbpos.z (int)sensor (int)body (int)dof | 17: armature - - -
+// Link-link contact (QLane<.., SELF = true>, collision filter 0; chain length 3 only) appends QSELF_F4 rows to the blob:
+//  S0: self_kn self_cn self_mu -        S1, S2 ([k][leg]): candidate words of own sphere a = 2 s + c (link s, slot c), a = 4 k + component
+//  word bits: [6 (p - 1) + b]  sphere b = 2 s' + c' of the leg on lane (lane ^ p), p = 1..3;  [18 + k]  the base's sphere k
+// and 2 NS park rows per thread: the world centres (about the base position) and radii of the lane's sphere slots.
 constexpr int QHDR_F4 = 19;
 constexpr int QL_F4 = 18;
 constexpr int QROOT_CP = 8;
 constexpr int QLINK_CP = 2;
 constexpr int QPOSE_F4 = 5;      // parked pose of a link: R(9) x(3) vw(3) vl(3)
-__host__ __device__ constexpr int quad_model_f4(int ns) { return QHDR_F4 + ns * QL_F4 * 4; }
-__host__ __device__ constexpr int quad_park_f4(int ns) { return ns * QPOSE_F4 + (ns - 1) * ACC_F4; }
+constexpr int QSELF_F4 = 9;
+__host__ __device__ constexpr int quad_model_f4(int ns, bool self = false) { return QHDR_F4 + ns * QL_F4 * 4 + (self ? QSELF_F4 : 0); }
+__host__ __device__ constexpr int quad_park_f4(int ns, bool self = false) { return ns * QPOSE_F4 + (ns - 1) * ACC_F4 + (self ? 2 * ns : 0); }
 
 B2G_HD float q_rsqrt(float x) {
 #ifdef __CUDA_ARCH__
@@ -51,6 +56,13 @@ B2G_HD float q_rcp(float x) {
     float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r;
 #else
     return 1.0f / x;
+#endif
+}
+B2G_HD int q_ctz(unsigned v) {
+#ifdef __CUDA_ARCH__
+    return __ffs(v) - 1;
+#else
+    return __builtin_ctz(v);
 #endif
 }
 B2G_HD int q_f2i(float f) {
@@ -72,7 +84,12 @@ struct QOutputs {
 //   bit 0  every chain link's inertia about its COM is axisymmetric (a 1 + bm u u^T: capsules, spheres, cylinders) --
 //          rows 9/10 of the link block then hold (u, a | bm) and the congruence R Ic R^T (45 ops) becomes a 1 + bm (R u)(R u)^T (18);
 //   bit 1  the base's inertia is axisymmetric AND its COM is at its origin: no first-moment terms at all.
-template <int NS, bool HF, int SP = 0>
+// SELF: link-link contact (the model's self_pairs, packed by quad_build).  A pre-pass parks every lane's link poses, twists
+// and sphere centres at the start of the sub-step; each lane then tests its own spheres against the other legs' (read from
+// their park columns) and the base's, and takes its own side of every overlapping pair -- both sides of a leg-leg pair are
+// computed, once on each lane, so nothing needs atomics or a hit list.  The base's side of a base-leg pair joins the leg
+// lane's share of the base before the butterfly.
+template <int NS, bool HF, int SP = 0, bool SELF = false>
 struct QLane {
     // accumulate-into-FMA forms: on for the 3-link chains (ANYmal: 196 registers, nothing spills), off for the 2-link Ant
     // kernel whose 128-register cap (14 warps per SM = one wave of 16384 envs) turns the longer live ranges into spills
@@ -261,6 +278,175 @@ struct QLane {
         x[0] = c.y; x[1] = c.z; x[2] = c.w; vw[0] = d.x; vw[1] = d.y; vw[2] = d.z; vl[0] = d.w; vl[1] = e.x; vl[2] = e.y;
     }
 
+    // ================= link-link contact (SELF)
+    static constexpr int SROW = NS * QPOSE_F4 + (NS - 1) * ACC_F4;   // first park row of the sphere centres
+    static constexpr int QS = QHDR_F4 + NS * QL_F4 * 4;              // first blob row of the self-collision table
+    // park row r of lane l of this env (the four lanes' columns are adjacent)
+    B2G_HD float4 &PKL(int l, int r) const { return park[(l - lane) + r * pstride]; }
+    B2G_HD unsigned self_word(int a) const {
+        return (unsigned)q_f2i(reinterpret_cast<const float *>(qm + QS + 1 + (a >> 2) * 4 + lane)[a & 3]);
+    }
+    // link masses as this env sees them (the per-env mass factor included)
+    B2G_HD float link_mass(int l, int s) const {
+        const float m = qm[QHDR_F4 + (s * QL_F4 + 10) * 4 + l].z;
+        return dr_mass ? m * dr_mass[q_f2i(qm[QHDR_F4 + (s * QL_F4 + 16) * 4 + l].w) + 1] : m;
+    }
+    B2G_HD float base_mass() const { return dr_mass ? qm[4].w * dr_mass[0] : qm[4].w; }
+
+    // kinematics pre-pass: pose and twist of every link of this lane's chain at the start of the sub-step (the rows the
+    // acceleration pass reads back), and the world centres of its sphere slots
+    B2G_HD void self_prepass(const RootState &rs) const {
+        float Rp[9]; quat_to_mat(rs.rq, Rp);
+        float xp[3] = {0.f, 0.f, 0.f}, vwp[3] = {rs.rw[0], rs.rw[1], rs.rw[2]}, vlp[3] = {rs.rv[0], rs.rv[1], rs.rv[2]};
+#pragma unroll
+        for (int s = 0; s < NS; s++) {
+            const float4 k0 = LK(s, 0), k1 = LK(s, 1), k2 = LK(s, 2), k3 = LK(s, 3), k4 = LK(s, 4), k5 = LK(s, 5), k6 = LK(s, 6), k7 = LK(s, 7), k8 = LK(s, 8);
+            float sn, cs; b2g_sincos(q[s], &sn, &cs);
+            const float Rj[9] = {k0.x + cs * k2.y + sn * k4.z, k0.y + cs * k2.z + sn * k4.w, k0.z + cs * k2.w + sn * k5.x,
+                                 k0.w + cs * k3.x + sn * k5.y, k1.x + cs * k3.y + sn * k5.z, k1.y + cs * k3.z + sn * k5.w,
+                                 k1.z + cs * k3.w + sn * k6.x, k1.w + cs * k4.x + sn * k6.y, k2.x + cs * k4.y + sn * k6.z};
+            float R[9]; matmul(Rp, Rj, R);
+            const float axp[3] = {k6.w, k7.x, k7.y}, lp[3] = {k7.z, k7.w, k8.x};
+            float x[3], ws[3], ss[3], vw[3], vl[3];
+            matvec(Rp, axp, ws);
+            matvec_add(Rp, lp, xp, x);
+            cross(x, ws, ss);
+#pragma unroll
+            for (int c = 0; c < 3; c++) { vw[c] = vwp[c] + ws[c] * qd[s]; vl[c] = vlp[c] + ss[c] * qd[s]; }
+            park_pose(s, R, x, vw, vl);
+#pragma unroll
+            for (int c = 0; c < 2; c++) {
+                const float4 cp = LK(s, 13 + c);
+                const float cpl[3] = {cp.x, cp.y, cp.z};
+                float pc[3]; matvec_add(R, cpl, x, pc);
+                PK(SROW + 2 * s + c) = make_float4(pc[0], pc[1], pc[2], cp.w);
+            }
+#pragma unroll
+            for (int c = 0; c < 9; c++) Rp[c] = R[c];
+#pragma unroll
+            for (int c = 0; c < 3; c++) { xp[c] = x[c]; vwp[c] = vw[c]; vlp[c] = vl[c]; }
+        }
+    }
+    // does sphere ci overlap sphere cj?  (the generic Stepper's test: coincident centres have no normal)
+    B2G_HD static bool self_overlap(const float4 ci, const float4 cj) {
+        const float dx = ci.x - cj.x, dy = ci.y - cj.y, dz = ci.z - cj.z, rsum = ci.w + cj.w;
+        const float d2 = dx * dx + dy * dy + dz * dz;
+        return d2 < rsum * rsum && d2 >= 1e-12f;
+    }
+    // one side of one overlapping pair: sphere ci of this body (mass mi, origin x, twist vw / vl) against sphere cj of a
+    // partner (mass mj, twist vwj / vlj at the start of the sub-step).  Gains from the reduced mass and the sub-step:
+    // kn = self_kn m_red / h^2, cn = self_cn m_red / h.  ACCUM: h J^T G J into I, -J^T F0 into the bias; !ACCUM: the force
+    // applied over the sub-step, F0 - h G (J a), and its torque about x, added to (F, T) -- as sphere() for the ground.
+    template <bool ACCUM>
+    B2G_HD void self_pair(const float4 ci, const float4 cj, float mi, float mj, const float x[3], const float vw[3], const float vl[3],
+                          const float vwj[3], const float vlj[3], float I[21], float pa[3], float pl[3],
+                          const float aw[3], const float al[3], float F[3], float T[3]) const {
+        const float4 S = qm[QS];
+        const float h = qm[0].x, vs2 = qm[1].z;
+        const float mred = mi * mj / (mi + mj);
+        const float skn = S.x * mred / (h * h), gn = S.y * mred / h + h * skn;
+        const float dv[3] = {ci.x - cj.x, ci.y - cj.y, ci.z - cj.z};
+        const float d2 = dot3(dv, dv), rsum = ci.w + cj.w;
+        const float inv = q_rsqrt(d2), dist = d2 * inv, pen = rsum - dist;
+        const float n[3] = {dv[0] * inv, dv[1] * inv, dv[2] * inv};                 // force on THIS body: away from the partner
+        const float off = ci.w - 0.5f * pen;                                         // contact point: middle of the overlap
+        const float r[3] = {ci.x - off * n[0], ci.y - off * n[1], ci.z - off * n[2]};
+        float ui[3], uj[3];
+        cross_add(vw, r, vl, ui); cross_add(vwj, r, vlj, uj);
+        const float rel[3] = {ui[0] - uj[0], ui[1] - uj[1], ui[2] - uj[2]};
+        const float un = dot3(rel, n);
+        const float Fn = skn * pen - gn * un;
+        if (Fn <= 0.f) return;
+        const float ut[3] = {rel[0] - un * n[0], rel[1] - un * n[1], rel[2] - un * n[2]};
+        const float gam = S.z * Fn * q_rsqrt(dot3(ut, ut) + vs2);
+        const float F0[3] = {Fn * n[0] - gam * ut[0], Fn * n[1] - gam * ut[1], Fn * n[2] - gam * ut[2]};
+        if (ACCUM) {
+            cross_sub<FACC>(r, F0, pa);
+            pl[0] -= F0[0]; pl[1] -= F0[1]; pl[2] -= F0[2];
+            const float hgam = h * gam;
+            const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
+            const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
+            sym6_rank1(I, hgam, jx, ex); sym6_rank1(I, hgam, jy, ey); sym6_rank1(I, hgam, jz, ez);
+            float rxn[3]; cross(r, n, rxn);
+            sym6_rank1(I, h * (gn - gam), rxn, n);
+        } else {
+            float Ja[3]; cross_add(aw, r, al, Ja);
+            const float Jan = dot3(Ja, n);
+            float Fk[3];
+#pragma unroll
+            for (int c = 0; c < 3; c++) Fk[c] = F0[c] - h * (gam * Ja[c] + (gn - gam) * Jan * n[c]);
+            const float rl[3] = {r[0] - x[0], r[1] - x[1], r[2] - x[2]};
+            cross_acc<FACC>(rl, Fk, T);
+#pragma unroll
+            for (int c = 0; c < 3; c++) F[c] += Fk[c];
+        }
+    }
+    // this lane's link s: its side of every overlapping pair of its spheres with the other legs' and the base's
+    template <bool ACCUM>
+    B2G_HD void self_link(int s, const RootState &rs, const float Rr[9], const float x[3], const float vw[3], const float vl[3],
+                          float I[21], float pa[3], float pl[3], const float aw[3], const float al[3], float F[3], float T[3]) const {
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+            unsigned bits = self_word(2 * s + c);
+            if (!bits) continue;
+            const float4 ci = PK(SROW + 2 * s + c);
+            const float mi = link_mass(lane, s);
+#pragma unroll 1
+            while (bits) {
+                const int b = q_ctz(bits);
+                bits &= bits - 1;
+                float4 cj;
+                int pln = -1;
+                if (b < 18) { pln = lane ^ (b / 6 + 1); cj = PKL(pln, SROW + b % 6); }
+                else {
+                    const float4 cp = qm[8 + b - 18];
+                    const float cpl[3] = {cp.x, cp.y, cp.z};
+                    float pc[3]; matvec(Rr, cpl, pc);
+                    cj = make_float4(pc[0], pc[1], pc[2], cp.w);
+                }
+                if (!self_overlap(ci, cj)) continue;
+                float vwj[3], vlj[3], mj;
+                if (pln >= 0) {
+                    const int ps = (b % 6) >> 1;
+                    const float4 t0 = PKL(pln, ps * QPOSE_F4 + 3), t1 = PKL(pln, ps * QPOSE_F4 + 4);
+                    vwj[0] = t0.x; vwj[1] = t0.y; vwj[2] = t0.z; vlj[0] = t0.w; vlj[1] = t1.x; vlj[2] = t1.y;
+                    mj = link_mass(pln, ps);
+                } else {
+#pragma unroll
+                    for (int k = 0; k < 3; k++) { vwj[k] = rs.rw[k]; vlj[k] = rs.rv[k]; }
+                    mj = base_mass();
+                }
+                self_pair<ACCUM>(ci, cj, mi, mj, x, vw, vl, vwj, vlj, I, pa, pl, aw, al, F, T);
+            }
+        }
+    }
+    // the base's side of the overlapping pairs of its spheres with this lane's leg (into this lane's share of the base)
+    template <bool ACCUM>
+    B2G_HD void self_base(const RootState &rs, const float Rr[9], float I[21], float pa[3], float pl[3],
+                          const float aw[3], const float al[3], float F[3], float T[3]) const {
+        const float xr[3] = {0.f, 0.f, 0.f};
+#pragma unroll 1
+        for (int a = 0; a < 2 * NS; a++) {
+            unsigned bits = self_word(a) >> 18;
+            if (!bits) continue;
+            const float4 cj = PK(SROW + a);
+            const int s = a >> 1;
+            const float4 t0 = PK(s * QPOSE_F4 + 3), t1 = PK(s * QPOSE_F4 + 4);
+            const float vwj[3] = {t0.x, t0.y, t0.z}, vlj[3] = {t0.w, t1.x, t1.y};
+#pragma unroll 1
+            while (bits) {
+                const int k = q_ctz(bits);
+                bits &= bits - 1;
+                const float4 cp = qm[8 + k];
+                const float cpl[3] = {cp.x, cp.y, cp.z};
+                float pc[3]; matvec(Rr, cpl, pc);
+                const float4 ci = make_float4(pc[0], pc[1], pc[2], cp.w);
+                if (!self_overlap(ci, cj)) continue;
+                self_pair<ACCUM>(ci, cj, base_mass(), link_mass(lane, s), xr, rs.rw, rs.rv, vwj, vlj, I, pa, pl, aw, al, F, T);
+            }
+        }
+    }
+
     // ================= sweeps root -> leaves -> root of this lane's chain, plus this lane's share of the base.
     // Out: the lane's contribution to the base's articulated inertia and bias (to be summed over the 4 lanes).
     // park_poses: the acceleration pass of this sub-step will need the link poses again (contact wrench outputs).
@@ -350,6 +536,10 @@ struct QLane {
                         if (c0.w >= 0.f) sphere<true>(c0, k15.x, rs.rp, R, x, vw, vl, I, qa, ql, dummy, dummy, dummy, dummy);
                         if (c1.w >= 0.f) sphere<true>(c1, k15.y, rs.rp, R, x, vw, vl, I, qa, ql, dummy, dummy, dummy, dummy);
                     }
+                }
+                if (SELF) {
+                    float dummy[3];
+                    self_link<true>(s, rs, Rr, x, vw, vl, I, qa, ql, dummy, dummy, dummy, dummy);
                 }
                 if (park_poses) park_pose(s, R, x, vw, vl);
                 if (s < NS - 1) {     // park the link's own terms until the leaf->root sweep comes back
@@ -479,6 +669,7 @@ struct QLane {
                 sphere<true>(cp, mu, rs.rp, Rr, xr, rs.rw, rs.rv, IA, pa, pl, dummy, dummy, dummy, dummy);
                 cp = cpn; mu = mun;
             }
+            if (SELF) self_base<true>(rs, Rr, IA, pa, pl, dummy, dummy, dummy, dummy);
         }
     }
 
@@ -495,6 +686,7 @@ struct QLane {
             const float mu = reinterpret_cast<const float *>(qm + 16)[k];
             sphere<false>(cp, mu, rs.rp, Rr, xr, rs.rw, rs.rv, dI, d3, d3, awr, alr, F, T);
         }
+        if (SELF) self_base<false>(rs, Rr, dI, d3, d3, awr, alr, F, T);
     }
     // force sensor (body frame, torque about the body origin) / net contact force of one link
     // keep (optional, 6 floats): the sensor reading also stays with the caller (the fused step kernels put it into the
@@ -547,6 +739,7 @@ struct QLane {
                     load_pose(s, R, x, vw, vl);
                     if (c0.w >= 0.f) sphere<false>(c0, k15.x, rs.rp, R, x, vw, vl, dI, d3, d3, aw, al, F, T);
                     if (c1.w >= 0.f) sphere<false>(c1, k15.y, rs.rp, R, x, vw, vl, dI, d3, d3, aw, al, F, T);
+                    if (SELF) { float Rr[9]; quat_to_mat(rs.rq, Rr); self_link<false>(s, rs, Rr, x, vw, vl, dI, d3, d3, aw, al, F, T); }
                     const float sb[3] = {k15.z, k15.w, k16.x};
                     emit(o, sensor, body, sb, R, F, T);
                 }
@@ -599,7 +792,12 @@ struct QLane {
     __device__ __forceinline__ void substep(RootState &rs, const bool LAST, const QOutputs &o) {
         float IA[21], pa[3], pl[3];
         const bool poses = LAST && needs_poses(o);
-        sweep(rs, poses, IA, pa, pl);
+        if (SELF) {                    // the partners' poses of the last sub-step are read; then this one's are
+            __syncwarp();
+            self_prepass(rs);
+            __syncwarp();
+        }
+        sweep(rs, SELF ? false : poses, IA, pa, pl);
 #pragma unroll
         for (int c = 0; c < 21; c++) IA[c] = lane_sum<4>(IA[c]);
 #pragma unroll

@@ -42,15 +42,19 @@ static inline bool quad_axisymmetric(const float I6[6], float u[3], float *a, fl
     return true;
 }
 
-// Returns the chain length NS (2 or 3) and fills `qm` (quad_model_f4(NS) float4, as floats) when the model fits the
+// Returns the chain length NS (2 or 3) and fills `qm` (quad_model_f4(NS, self) float4, as floats) when the model fits the
 // quad path; 0 otherwise (the generic Stepper handles it).  leg_link[l * NS + s] = link of lane l, slot s.
 // *spec receives the QLane specialisation flags the packed constants are laid out for (0 or 3; want_spec = 0 forces the
-// general layout).
+// general layout).  A self-colliding model (m->self_collide) fits for chain length 3 only, in the general layout, and only
+// when no candidate pair lies within one leg; its self-collision table follows the link table (b2g_quad.cuh).
 static inline int quad_build(const b2g_model *m, const b2g_sim_params *sp, std::vector<float> &qm, int leg_link[12], int *spec = nullptr, int want_spec = 3) {
     if (m->root_fixed || m->nl < 9) return 0;
     const int nd = m->nl - 1;
     if (nd != 8 && nd != 12) return 0;
     const int NS = nd / 4;
+    const bool self = m->self_collide && m->self_pairs;
+    if (self && NS != 3) return 0;
+    if (self) want_spec = 0;
     int roots[4], nroot = 0;
     for (int i = 1; i < m->nl; i++) if (m->parent[i] == 0) { if (nroot == 4) return 0; roots[nroot++] = i; }
     if (nroot != 4) return 0;
@@ -90,7 +94,8 @@ static inline int quad_build(const b2g_model *m, const b2g_sim_params *sp, std::
     }
     if (spec) *spec = sflags;
 
-    qm.assign((size_t)quad_model_f4(NS) * 4, 0.f);
+    qm.assign((size_t)quad_model_f4(NS, self) * 4, 0.f);
+    std::vector<int> sph_lane(m->ncp, -1), sph_slot(m->ncp, 0);     // contact sphere -> (lane, 2 s + c), or (-1, base slot)
     auto F4 = [&](int idx) { return qm.data() + 4 * (size_t)idx; };
     const float h = sp->dt / (float)sp->substeps;
     float g[3];
@@ -123,6 +128,7 @@ static inline int quad_build(const b2g_model *m, const b2g_sim_params *sp, std::
             float *P = F4(8 + k0);
             P[0] = m->cp_pos[3 * k]; P[1] = m->cp_pos[3 * k + 1]; P[2] = m->cp_pos[3 * k + 2]; P[3] = m->cp_radius[k];
             F4(16)[k0] = 0.5f * (m->cp_mu[k] + sp->ground_friction);
+            sph_slot[k] = k0;
             k0++;
         }
     }
@@ -166,12 +172,32 @@ static inline int quad_build(const b2g_model *m, const b2g_sim_params *sp, std::
             float *P = L + 52 + 4 * k0;
             P[0] = m->cp_pos[3 * k]; P[1] = m->cp_pos[3 * k + 1]; P[2] = m->cp_pos[3 * k + 2]; P[3] = m->cp_radius[k];
             L[60 + k0] = 0.5f * (m->cp_mu[k] + sp->ground_friction);
+            sph_lane[k] = l; sph_slot[k] = 2 * s + k0;
             k0++;
         }
         if (link_sensor[li] >= 0) { const float *bp = m->body_pos + 3 * m->sensor_body[link_sensor[li]]; L[62] = bp[0]; L[63] = bp[1]; L[64] = bp[2]; }
         L[65] = q_i2f(link_sensor[li]); L[66] = q_i2f(link_body[li]); L[67] = q_i2f(li - 1);
         L[68] = m->armature[li];
         for (int k = 0; k < QL_F4; k++) memcpy(F4(QHDR_F4 + (s * QL_F4 + k) * 4 + l), L + 4 * k, 16);
+    }
+    if (self) {
+        const int QS = QHDR_F4 + NS * QL_F4 * 4;
+        { float *S = F4(QS); S[0] = m->self_kn; S[1] = m->self_cn; S[2] = m->self_mu; }
+        unsigned word[4][8] = {};
+        for (int i = 0; i < m->ncp; i++) for (int j = i + 1; j < m->ncp; j++) {
+            if (!m->self_pairs[(size_t)i * m->ncp + j] && !m->self_pairs[(size_t)j * m->ncp + i]) continue;
+            const int li = sph_lane[i], lj = sph_lane[j], ai = sph_slot[i], aj = sph_slot[j];
+            if (li < 0 && lj < 0) continue;                                  // both on the base: one link
+            if (li == lj) return 0;                                          // within one leg: the generic Stepper
+            if (li < 0) word[lj][aj] |= 1u << (18 + ai);
+            else if (lj < 0) word[li][ai] |= 1u << (18 + aj);
+            else {
+                const int p = li ^ lj;
+                word[li][ai] |= 1u << (6 * (p - 1) + aj);
+                word[lj][aj] |= 1u << (6 * (p - 1) + ai);
+            }
+        }
+        for (int l = 0; l < 4; l++) for (int a = 0; a < 2 * NS; a++) F4(QS + 1 + (a >> 2) * 4 + l)[a & 3] = q_i2f((int)word[l][a]);
     }
     return NS;
 }

@@ -10,9 +10,9 @@
 namespace b2g {
 
 // dynamic shared memory of the quad kernels: [park: quad_park_f4(NS) x BLOCK float4][tiles ...][quad model]
-template <int NS, bool HF, int SP>
-__device__ __forceinline__ QLane<NS, HF, SP> make_qlane(const float4 *qm, const int16_t *hf, float4 *park_base, int block, int lane) {
-    QLane<NS, HF, SP> L;
+template <int NS, bool HF, int SP, bool SELF = false>
+__device__ __forceinline__ QLane<NS, HF, SP, SELF> make_qlane(const float4 *qm, const int16_t *hf, float4 *park_base, int block, int lane) {
+    QLane<NS, HF, SP, SELF> L;
     L.qm = qm; L.hf = hf; L.park = park_base + threadIdx.x; L.pstride = block; L.lane = lane; L.env_mu = -1.f;
     L.dr_mass = nullptr; L.dr_dof = nullptr;
     return L;
@@ -29,18 +29,19 @@ __device__ __forceinline__ void attach_env_params(QL &L, const Buffers &B, int e
     if (envmu) L.env_mu = 0.5f * (envmu[e] + L.qm[18].x);             // PhysX default combine mode: the average of the two materials
 }
 
-template <int NS, bool HF, int SP, int BLOCK>
+// SELF: link-link contact (a self-colliding model; its blob and park area are larger, see b2g_quad.cuh)
+template <int NS, bool HF, int SP, int BLOCK, bool SELF = false>
 __global__ void __launch_bounds__(BLOCK) quad_simulate_kernel(const float4 *__restrict__ gqm, const int16_t *__restrict__ hf, Buffers B, int N, int substeps) {
     float4 *const park = b2g_dyn_smem;
-    float4 *const qm = b2g_dyn_smem + quad_park_f4(NS) * BLOCK;
-    for (int i = threadIdx.x; i < quad_model_f4(NS); i += BLOCK) qm[i] = gqm[i];
+    float4 *const qm = b2g_dyn_smem + quad_park_f4(NS, SELF) * BLOCK;
+    for (int i = threadIdx.x; i < quad_model_f4(NS, SELF); i += BLOCK) qm[i] = gqm[i];
     __syncthreads();
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt >> 2, lane = gt & 3;
     const bool valid = env < N;
     const int e = valid ? env : N - 1;
     constexpr int nd = 4 * NS;
-    QLane<NS, HF, SP> L = make_qlane<NS, HF, SP>(qm, hf, park, BLOCK, lane);
+    QLane<NS, HF, SP, SELF> L = make_qlane<NS, HF, SP, SELF>(qm, hf, park, BLOCK, lane);
     attach_env_params(L, B, e, nd);
     float *const root_row = (float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e;
     RootState rs; load_root(root_row, rs);
@@ -343,21 +344,22 @@ __global__ void __launch_bounds__(BLOCK, B2G_QUAD_MINBLOCKS(BLOCK)) quad_loco_ke
 // the 5 sub-steps; the PD law reads it there.
 // DR = false: no per-env link-mass / joint-property arrays bound -- their pointers are compile-time nulls (smaller code: this kernel runs one
 // warp per scheduler, so instruction fetch is exposed: 27 % of its stall cycles are "no instruction")
-template <bool HF, int BLOCK, bool DR = true>
+// SELF: link-link contact (env.selfCollision; the model's self-collision table follows the link table)
+template <bool HF, int BLOCK, bool DR = true, bool SELF = false>
 __global__ void __launch_bounds__(BLOCK) quad_anymal_physics_kernel(const float4 *__restrict__ gqm, const int16_t *__restrict__ hf,
                                                                     Buffers B, const __grid_constant__ b2g_anymal_params P,
                                                                     const float *__restrict__ actions_in, int N, int substeps, unsigned step_counter) {
     constexpr int NS = 3, nd = 12;
     __shared__ float s_part[BLOCK / 32];
     float4 *const park = b2g_dyn_smem;
-    float4 *const qm = b2g_dyn_smem + quad_park_f4(NS) * BLOCK;
-    for (int i = threadIdx.x; i < quad_model_f4(NS); i += BLOCK) qm[i] = gqm[i];
+    float4 *const qm = b2g_dyn_smem + quad_park_f4(NS, SELF) * BLOCK;
+    for (int i = threadIdx.x; i < quad_model_f4(NS, SELF); i += BLOCK) qm[i] = gqm[i];
     __syncthreads();
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt >> 2, lane = gt & 3;
     const bool valid = env < N;
     const int e = valid ? env : N - 1;
-    QLane<NS, HF, 0> L = make_qlane<NS, HF, 0>(qm, hf, park, BLOCK, lane);
+    QLane<NS, HF, 0, SELF> L = make_qlane<NS, HF, 0, SELF>(qm, hf, park, BLOCK, lane);
     attach_env_params(L, B, e, nd, DR);                      // the per-env friction (terrain buckets, anymal_terrain.py:238-247) is always honoured
     RootState rs; load_root((const float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
     const float2 *dofs = (const float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;

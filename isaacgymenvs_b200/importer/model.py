@@ -333,9 +333,10 @@ def enable_self_collision(m: "Model", kappa=0.5, zeta=0.5, mu=1.0, samples=4096,
 
 
 def self_collision_supported(m: "Model"):
-    """Which models the engine's link-link contact covers: the generic sub-step, <= 64 contact spheres, <= 32 links.  A free base
-    with four identical hinge chains (Ant, ANYmal) runs on the four-chain kernels, which do not carry it: such a model keeps
-    its speed and says so (engine.warn_self_collision) instead."""
+    """Which models the compatibility path (compat/gymapi.py create_actor with filter 0) turns link-link contact on for: the
+    generic sub-step, <= 64 contact spheres, <= 32 links.  A free base with four identical hinge chains (Ant, ANYmal) is left
+    out here and says so (engine.warn_self_collision): the Ant's runs on the generic sub-step, and the four-chain kernels
+    carry ANYmal's (AnymalTerrain's env.selfCollision), but turning it on by default would change this path's outputs."""
     if len(m.cp_link) > 64 or m.nl > 32:
         return False
     if not m.root_fixed and m.ndof in (8, 12):

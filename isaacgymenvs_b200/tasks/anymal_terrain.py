@@ -6,7 +6,7 @@ import torch
 
 from .. import engine
 from ..assets import load_asset_file
-from ..importer.model import BuildOptions, DRIVE_EFFORT
+from ..importer.model import BuildOptions, DRIVE_EFFORT, enable_self_collision
 from ..terrain import Terrain
 from .base.vec_task import VecTask
 from .locomotion import _asset_root
@@ -67,7 +67,12 @@ class AnymalTerrain(VecTask):
         opts = BuildOptions(collapse_fixed_joints=True, replace_cylinder_with_capsule=True, density=0.001,
                             fix_base_link=e["urdfAsset"]["fixBaseLink"], default_dof_drive_mode=DRIVE_EFFORT)
         model = copy.deepcopy(load_asset_file(_asset_root(), e["urdfAsset"]["file"], opts))
-        engine.warn_self_collision("AnymalTerrain", "anymal_terrain.py:282 create_actor(..., i, 0, 0)")
+        # anymal_terrain.py:282 create_actor(..., i, 0, 0): collision filter 0 = the legs collide with each other and the base
+        # (env.selfCollision: True = as the reference, on the four-chain kernels; default False = without it, announced by a warning)
+        if e.get("selfCollision", False):
+            enable_self_collision(model)
+        else:
+            engine.warn_self_collision("AnymalTerrain", "anymal_terrain.py:282 create_actor(..., i, 0, 0); set env.selfCollision=True to model it")
         self.num_dof, self.num_bodies = model.ndof, model.nb
         self.dof_names = list(model.dof_names)
         body_names = list(model.body_names)

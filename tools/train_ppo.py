@@ -79,7 +79,7 @@ def main(argv=None):
     ap.add_argument("--lr", type=float, default=3e-4)          # HumanoidPPO.yaml: 5e-4
     ap.add_argument("--mini-epochs", type=int, default=4)      # HumanoidPPO.yaml: 5
     ap.add_argument("--critic-coef", type=float, default=2.0)  # HumanoidPPO.yaml: 4
-    ap.add_argument("--self-collision", action="store_true")   # Humanoid: env.selfCollision=True
+    ap.add_argument("--self-collision", action="store_true")   # Humanoid, AnymalTerrain: env.selfCollision=True
     ap.add_argument("--kl-threshold", type=float, default=0.008)   # ShadowHandPPO.yaml: 0.016
     ap.add_argument("--reward-scale", type=float, default=0.01)    # reward_shaper.scale_value; CartpolePPO.yaml 0.1, AnymalTerrainPPO.yaml 1.0
     ap.add_argument("--bounds-coef", type=float, default=1e-4)     # bounds_loss_coef; AnymalTerrainPPO.yaml 0
