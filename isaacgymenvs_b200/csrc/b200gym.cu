@@ -1018,7 +1018,7 @@ static int launch_anymal_physics(b2g_sim *s, const b2g_anymal_params &P, const f
     }
     // the generic AnymalTerrain kernel has no link-link contact: never drop it silently
     if (self) return fail(B2G_E_UNSUPPORTED, "b2g_task_step(AnymalTerrain): link-link contact needs the four-chain kernels (unset B2G_NO_QUAD)");
-    const auto k = hf ? anymal_physics_kernel<4, true, 128> : anymal_physics_kernel<4, false, 128>;
+    const auto k = hf ? anymal_physics_kernel<true> : anymal_physics_kernel<false>;
     return launch(s, k, grid, 128, s->dyn_smem, st, SMEM, s->dm, s->d_hf, s->buf, P, actions, N, s->step_counter);
 }
 
@@ -1040,7 +1040,7 @@ static int anymal_step(b2g_sim *s, const float *actions, void *stream) {
     rc = launch_anymal_physics(s, P, actions, N, grid, st); if (rc) return rc;
     // kernel 2: one WARP per env -- the 140-point height gather (anymal_terrain.py:515-538) and the 188 observation
     // stores dominate it; with 4 lanes per env the 4096-env workload was 512 warps on 592 schedulers
-    return launch(s, anymal_reset_obs_kernel<32, 128>, (N * 32 + 127) / 128, 128, 0, st, PLAIN,
+    return launch(s, anymal_reset_obs_kernel, (N * 32 + 127) / 128, 128, 0, st, PLAIN,
                   s->buf, P, s->d_hf, N, s->hm.nl - 1, grid, s->step_counter, 0);
 }
 
@@ -1218,7 +1218,7 @@ extern "C" int b2g_reset_flagged(b2g_sim *s, void *stream) {
         rc = require(s, {B2G_T_COMMANDS, B2G_T_FEET_AIR_TIME, B2G_T_EPISODE_SUMS, B2G_T_REDUCE_SCRATCH}, "b2g_reset_flagged(AnymalTerrain)"); if (rc) return rc;
         if (s->anymal.custom_origins) { rc = require(s, {B2G_T_ENV_ORIGINS, B2G_T_TERRAIN_LEVELS, B2G_T_TERRAIN_TYPES, B2G_T_TERRAIN_ORIGINS}, "b2g_reset_flagged(AnymalTerrain)"); if (rc) return rc; }
         CUDA_TRY(cudaMemsetAsync((float *)s->buf.p[B2G_T_REDUCE_SCRATCH] + REDUCE_PARTIALS, 0, 16 * sizeof(float), st));
-        return launch(s, anymal_reset_obs_kernel<32, 128>, (N * 32 + 127) / 128, 128, 0, st, PLAIN, s->buf, s->anymal, s->d_hf, N, nd, 0, s->step_counter, 1);
+        return launch(s, anymal_reset_obs_kernel, (N * 32 + 127) / 128, 128, 0, st, PLAIN, s->buf, s->anymal, s->d_hf, N, nd, 0, s->step_counter, 1);
     }
     if (s->has_hand) {
         rc = require(s, {B2G_T_INITIAL_ROOT, B2G_T_GOAL_STATES, B2G_T_DOF_TARGET, B2G_T_PREV_TARGETS, B2G_T_SUCCESSES, B2G_T_RESET_GOAL}, "b2g_reset_flagged(ShadowHand)"); if (rc) return rc;

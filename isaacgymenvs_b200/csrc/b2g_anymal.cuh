@@ -15,10 +15,12 @@
 
 namespace b2g {
 
-template <int L, bool HF, int BLOCK>
-__global__ void __launch_bounds__(BLOCK) anymal_physics_kernel(const DevModel *__restrict__ gm, const int16_t *__restrict__ hf,
-                                                                Buffers B, const __grid_constant__ b2g_anymal_params P,
-                                                                const float *__restrict__ actions_in, int N, unsigned step_counter) {
+// four lanes per env on the generic Stepper (lane k owns leg k), 128 threads
+template <bool HF>
+__global__ void __launch_bounds__(128) anymal_physics_kernel(const DevModel *__restrict__ gm, const int16_t *__restrict__ hf,
+                                                              Buffers B, const __grid_constant__ b2g_anymal_params P,
+                                                              const float *__restrict__ actions_in, int N, unsigned step_counter) {
+    constexpr int L = 4, BLOCK = 128;
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
     __shared__ float s_part[BLOCK / 32];
@@ -60,9 +62,7 @@ __global__ void __launch_bounds__(BLOCK) anymal_physics_kernel(const DevModel *_
                 const int d = st.link_of(s) - 1;
                 if (d < 0) continue;
                 const float2 qv = st.get_q(s);
-                const float a = act_out[(size_t)e * nd + d];
-                float t = P.kp * (P.action_scale * a + P.default_dof_pos[d] - qv.x) - P.kd * qv.y;
-                t = fminf(fmaxf(t, -P.torque_limit), P.torque_limit);
+                const float t = anymal_pd_torque(P, d, act_out[(size_t)e * nd + d], qv.x, qv.y);
                 st.set_act(s, t);
                 if (valid) torq[d] = t;
             }
@@ -71,128 +71,25 @@ __global__ void __launch_bounds__(BLOCK) anymal_physics_kernel(const DevModel *_
     }
 
     // ---- post_physics_step (:453-475)
-    long long *progress_b = (long long *)B.p[B2G_T_PROGRESS];
-    long long *reset_b = (long long *)B.p[B2G_T_RESET];
-    const long long progress = progress_b[e] + 1;
-    const uint32_t gid = (uint32_t)(e + P.env_id_offset);
-    if (P.push_robots && P.push_interval > 0 && (step_counter % (unsigned)P.push_interval) == 0) {   // push_robots :437-439
-        rs.rv[0] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 0));
-        rs.rv[1] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 1));
-    }
-    float2 *dw = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
-    // per-DOF reward sums of this lane (:339,342,355,361)
-    float s_torque = 0.f, s_jacc = 0.f, s_arate = 0.f, s_hip = 0.f;
+    anymal_post_physics<BLOCK>(P, B, N, e, lane, valid, step_counter, rs, o.net_contact, s_part, [&](AnymalCosts &c) {
+        float2 *dw = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
 #pragma unroll 1
-    for (int s = 0; s < NS; s++) {
-        const int d = st.link_of(s) - 1;
-        if (d < 0) continue;
-        const float2 qv = st.get_q(s);
-        if (valid) dw[d] = qv;
-        const float t = torq[d], a = act_out[(size_t)e * nd + d];
-        s_torque += t * t;
-        const float dv = last_v[d] - qv.y; s_jacc += dv * dv;
-        const float da = last_a[d] - a; s_arate += da * da;
-        if (d % 3 == 0) s_hip += fabsf(qv.x - P.default_dof_pos[d]);          // dof_pos[:, [0,3,6,9]]
-    }
-    if (valid && lane == 0 && !sm.root_fixed) store_root((float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
-    s_torque = lane_sum<L>(s_torque); s_jacc = lane_sum<L>(s_jacc); s_arate = lane_sum<L>(s_arate); s_hip = lane_sum<L>(s_hip);
-
-    // contact-force terms: every lane looks at bodies base / knee[lane] / foot[lane]
-    const float *cf = o.net_contact;
-    float *fat_b = (float *)B.p[B2G_T_FEET_AIR_TIME] + (size_t)e * 4;
-    float n_knee = 0.f, n_stumble = 0.f, air = 0.f;
-    bool knee_hit = false;
-    __syncwarp();
-    for (int k = lane; k < 4; k += L) {
-        const float *fk = cf + 3 * P.knee_bodies[k], *ff = cf + 3 * P.feet_bodies[k];
-        const bool kc = sqrtf(fk[0] * fk[0] + fk[1] * fk[1] + fk[2] * fk[2]) > 1.f;
-        knee_hit = knee_hit || kc;
-        n_knee += kc ? 1.f : 0.f;
-        n_stumble += ((sqrtf(ff[0] * ff[0] + ff[1] * ff[1]) > 5.f) && (fabsf(ff[2]) < 1.f)) ? 1.f : 0.f;
-        const bool contact = ff[2] > 1.f;
-        float fat = fat_b[k];
-        const bool first = (fat > 0.f) && contact;
-        fat += P.dt;
-        air += (fat - 0.5f) * (first ? 1.f : 0.f);
-        fat = contact ? 0.f : fat;
-        if (valid) fat_b[k] = fat;
-    }
-    n_knee = lane_sum<L>(n_knee); n_stumble = lane_sum<L>(n_stumble); air = lane_sum<L>(air);
-    const float any_knee = lane_sum<L>(knee_hit ? 1.f : 0.f);
-
-    // prepare quantities (:464-471)
-    float *cmd = (float *)B.p[B2G_T_COMMANDS] + (size_t)e * 4;
-    const float gvec[3] = {0.f, 0.f, -1.f}, fvec[3] = {1.f, 0.f, 0.f};
-    float blv[3], bav[3], pg[3], fwd[3];
-    t_quat_rotate(rs.rq, rs.rv, blv, -1.f);
-    t_quat_rotate(rs.rq, rs.rw, bav, -1.f);
-    t_quat_rotate(rs.rq, gvec, pg, -1.f);
-    t_quat_apply(rs.rq, fvec, fwd);
-    const float heading = atan2f(fwd[1], fwd[0]);
-    const float c0 = cmd[0], c1 = cmd[1], c3 = cmd[3];
-    const float c2 = fminf(fmaxf(0.5f * t_wrap_to_pi(c3 - heading), -1.f), 1.f);
-
-    // check_termination (:294-300)
-    const float *fb = cf + 3 * P.base_body;
-    bool reset = sqrtf(fb[0] * fb[0] + fb[1] * fb[1] + fb[2] * fb[2]) > 1.f;
-    if (!P.allow_knee_contacts) reset = reset || (any_knee > 0.f);
-    if (progress >= (long long)P.max_episode_length - 1) reset = true;
-
-    float part = 0.f;
-    if (lane == 0 && valid) {
-        // compute_reward (:315-382)
-        const float *R = P.rew_scales;
-        const float ex = c0 - blv[0], ey = c1 - blv[1];
-        const float lin_err = ex * ex + ey * ey;
-        const float ang_err = (c2 - bav[2]) * (c2 - bav[2]);
-        float t[13];
-        t[0] = expf(-lin_err / 0.25f) * R[1];                    // lin_vel_xy
-        t[1] = blv[2] * blv[2] * R[2];                           // lin_vel_z
-        t[2] = expf(-ang_err / 0.25f) * R[3];                    // ang_vel_z
-        t[3] = (bav[0] * bav[0] + bav[1] * bav[1]) * R[4];       // ang_vel_xy
-        t[4] = (pg[0] * pg[0] + pg[1] * pg[1]) * R[5];           // orient
-        t[5] = s_torque * R[6];                                  // torques
-        t[6] = s_jacc * R[7];                                    // joint_acc
-        t[7] = (rs.rp[2] - 0.52f) * (rs.rp[2] - 0.52f) * R[8];   // base_height
-        t[8] = air * R[9] * ((sqrtf(c0 * c0 + c1 * c1) > 0.1f) ? 1.f : 0.f);   // air_time
-        t[9] = n_knee * R[10];                                   // collision
-        t[10] = n_stumble * R[11];                               // stumble
-        t[11] = s_arate * R[12];                                 // action_rate
-        t[12] = s_hip * R[13];                                   // hip
-        float rew = t[0] + t[2] + t[1] + t[3] + t[4] + t[7] + t[5] + t[6] + t[9] + t[11] + t[8] + t[12] + t[10];
-        rew = fmaxf(rew, 0.f);
-        const uint8_t *to = (const uint8_t *)B.p[B2G_T_TIMEOUT];
-        rew += R[0] * (reset ? 1.f : 0.f) * ((to && to[e]) ? 0.f : 1.f);
-        ((float *)B.p[B2G_T_REW])[e] = rew;
-        float *es = (float *)B.p[B2G_T_EPISODE_SUMS];
-#pragma unroll
-        for (int k = 0; k < 13; k++) es[(size_t)k * N + e] += t[k];
-        reset_b[e] = reset ? 1 : 0;
-        progress_b[e] = progress;
-        cmd[2] = c2;
-        float *bs = (float *)B.p[B2G_T_BASE_SCRATCH] + (size_t)e * 12;
-        bs[0] = blv[0]; bs[1] = blv[1]; bs[2] = blv[2]; bs[3] = bav[0]; bs[4] = bav[1]; bs[5] = bav[2];
-        bs[6] = pg[0]; bs[7] = pg[1]; bs[8] = pg[2];
-        if (reset) part = c0 * c0 + c1 * c1;
-    }
-    // deterministic per-block partial of sum over the reset set of |commands_xy|^2
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
-    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = part;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int w = 0; w < BLOCK / 32; w++) tot += s_part[w];
-        float *red = (float *)B.p[B2G_T_REDUCE_SCRATCH];
-        red[blockIdx.x] = tot;
-        if (blockIdx.x == 0) for (int k = 0; k < 16; k++) red[REDUCE_PARTIALS + k] = 0.f;
-    }
+        for (int s = 0; s < NS; s++) {
+            const int d = st.link_of(s) - 1;
+            if (d < 0) continue;
+            const float2 qv = st.get_q(s);
+            if (valid) dw[d] = qv;
+            c.add(P, d, torq[d], act_out[(size_t)e * nd + d], qv.x, qv.y, last_a, last_v);
+        }
+        if (valid && lane == 0 && !sm.root_fixed) store_root((float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
+    });
 }
 
-template <int L, int BLOCK>
-__global__ void __launch_bounds__(BLOCK) anymal_reset_obs_kernel(Buffers B, const __grid_constant__ b2g_anymal_params P,
-                                                                  const int16_t *__restrict__ hs, int N, int nd,
-                                                                  int nblocks1, unsigned step_counter, int reset_only) {
+// one warp per env, 128 threads
+__global__ void __launch_bounds__(128) anymal_reset_obs_kernel(Buffers B, const __grid_constant__ b2g_anymal_params P,
+                                                                const int16_t *__restrict__ hs, int N, int nd,
+                                                                int nblocks1, unsigned step_counter, int reset_only) {
+    constexpr int L = 32, BLOCK = 128;
     // reset_only (VecTask.reset_done, vec_task.py:440-455 -> reset_idx :384-425 of the flagged envs, no step): the norm
     // over the reset set is summed here from the flags themselves; observations and last_* are left to the next step
     __shared__ float s_norm;
@@ -281,13 +178,12 @@ __global__ void __launch_bounds__(BLOCK) anymal_reset_obs_kernel(Buffers B, cons
     obsc = (obsc && obsc != (float *)B.p[B2G_T_OBS]) ? obsc + (size_t)e * P.num_obs : nullptr;
     const float *nsv = (const float *)B.p[B2G_T_NOISE_SCALE];
     // observation noise (:481-482): uniform number idx of stream (env, step); one Philox block serves 4 neighbours.
-    // Warp-per-env layout: the env's 47 Philox blocks are generated ONCE, spread over the 32 lanes (<= 2 each), and the
-    // noise terms parked in shared memory -- with each lane generating the blocks of the indices it happens to write, the
-    // Philox rounds were most of this kernel's instructions.  Narrower layouts keep the per-lane block cache.
-    constexpr bool WARP_ENV = (L == 32);
-    __shared__ float s_noise[WARP_ENV ? BLOCK / 32 : 1][WARP_ENV ? 192 : 1];
-    float *const my_noise = s_noise[WARP_ENV ? (threadIdx.x >> 5) : 0];
-    if (WARP_ENV && P.add_noise) {
+    // The env's 47 Philox blocks are generated ONCE, spread over the 32 lanes (<= 2 each), and the noise terms parked in
+    // shared memory -- with each lane generating the blocks of the indices it happens to write, the Philox rounds were
+    // most of this kernel's instructions.
+    __shared__ float s_noise[BLOCK / 32][192];
+    float *const my_noise = s_noise[threadIdx.x >> 5];
+    if (P.add_noise) {
         for (int blk = lane; 4 * blk < P.num_obs && blk < 48; blk += 32) {
             uint32_t r4[4];
             philox4x32_10((uint32_t)blk, step_counter, gid, TAG_NOISE, (uint32_t)P.seed, (uint32_t)(P.seed >> 32), r4);
@@ -299,20 +195,8 @@ __global__ void __launch_bounds__(BLOCK) anymal_reset_obs_kernel(Buffers B, cons
         }
         __syncwarp();
     }
-    uint32_t nz[4]; int nz_blk = -1;
     auto put = [&](int idx, float v) {
-        if (P.add_noise) {
-            if (WARP_ENV) {
-                v += my_noise[idx];
-            } else {
-                if ((idx >> 2) != nz_blk) {
-                    nz_blk = idx >> 2;
-                    philox4x32_10((uint32_t)nz_blk, step_counter, gid, TAG_NOISE, (uint32_t)P.seed, (uint32_t)(P.seed >> 32), nz);
-                }
-                const float u = (float)(nz[idx & 3] >> 8) * (1.0f / 16777216.0f);
-                v += (2.f * u - 1.f) * nsv[idx];
-            }
-        }
+        if (P.add_noise) v += my_noise[idx];
         obs[idx] = v;
         if (obsc) obsc[idx] = fminf(fmaxf(v, -P.clip_obs), P.clip_obs);
     };
@@ -383,8 +267,7 @@ __global__ void __launch_bounds__(BLOCK) anymal_reset_obs_kernel(Buffers B, cons
     // 15 ticket, [16,29) means, 29 mean terrain level, 32 running sum of terrain_levels.
     __syncwarp();
     if ((threadIdx.x & 31) == 0) {
-        const int first_env = blockIdx.x * (BLOCK / L);
-        const int nwarps = min(BLOCK / 32, (N - first_env) * (L / 32));            // warps of this block that own an env (L == 32)
+        const int nwarps = min(BLOCK / 32, N - (int)blockIdx.x * (BLOCK / 32));    // warps of this block that own an env
         // (no grid-scope fence here: only the few warps that reset an env touched the sums, and they fenced there; a
         // __threadfence by every warp invalidates L1 4096 times per launch -- measured +13 us)
         if (atomicAdd(&s_done, 1) == nwarps - 1) {

@@ -387,8 +387,7 @@ __global__ void __launch_bounds__(BLOCK) quad_anymal_physics_kernel(const float4
         if (k < pd_until && (k % substeps) == 0) {
 #pragma unroll
             for (int s = 0; s < NS; s++) {
-                float t = P.kp * (P.action_scale * a_cl[s] + P.default_dof_pos[dofi[s]] - L.q[s]) - P.kd * L.qd[s];
-                t = fminf(fmaxf(t, -P.torque_limit), P.torque_limit);
+                const float t = anymal_pd_torque(P, dofi[s], a_cl[s], L.q[s], L.qd[s]);
                 L.act[s] = t; tq[s] = t;
             }
         }
@@ -396,120 +395,16 @@ __global__ void __launch_bounds__(BLOCK) quad_anymal_physics_kernel(const float4
     }
 
     // ---- post_physics_step (:453-475)
-    long long *progress_b = (long long *)B.p[B2G_T_PROGRESS];
-    long long *reset_b = (long long *)B.p[B2G_T_RESET];
-    const long long progress = progress_b[e] + 1;
-    const uint32_t gid = (uint32_t)(e + P.env_id_offset);
-    if (P.push_robots && P.push_interval > 0 && (step_counter % (unsigned)P.push_interval) == 0) {   // push_robots :437-439
-        rs.rv[0] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 0));
-        rs.rv[1] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 1));
-    }
-    float2 *dw = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
-    float s_torque = 0.f, s_jacc = 0.f, s_arate = 0.f, s_hip = 0.f;
+    anymal_post_physics<BLOCK>(P, B, N, e, lane, valid, step_counter, rs, o.net_contact, s_part, [&](AnymalCosts &c) {
+        float2 *dw = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
 #pragma unroll
-    for (int s = 0; s < NS; s++) {
-        const int d = dofi[s];
-        if (valid) { dw[d] = make_float2(L.q[s], L.qd[s]); if (total > 0 && pd_until > 0) torq[d] = tq[s]; }
-        const float t = (total > 0 && pd_until > 0) ? tq[s] : torq[d], a = a_cl[s];
-        s_torque += t * t;
-        const float dv = last_v[d] - L.qd[s]; s_jacc += dv * dv;
-        const float da = last_a[d] - a; s_arate += da * da;
-        if (d % 3 == 0) s_hip += fabsf(L.q[s] - P.default_dof_pos[d]);          // dof_pos[:, [0,3,6,9]]
-    }
-    if (valid && lane == 0) store_root((float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
-    s_torque = lane_sum<4>(s_torque); s_jacc = lane_sum<4>(s_jacc); s_arate = lane_sum<4>(s_arate); s_hip = lane_sum<4>(s_hip);
-
-    // contact-force terms: every lane looks at bodies base / knee[lane] / foot[lane]
-    const float *cf = o.net_contact;
-    float *fat_b = (float *)B.p[B2G_T_FEET_AIR_TIME] + (size_t)e * 4;
-    float n_knee = 0.f, n_stumble = 0.f, air = 0.f;
-    bool knee_hit = false;
-    __syncwarp();
-    {
-        const int k = lane;
-        const float *fk = cf + 3 * P.knee_bodies[k], *ff = cf + 3 * P.feet_bodies[k];
-        const bool kc = sqrtf(fk[0] * fk[0] + fk[1] * fk[1] + fk[2] * fk[2]) > 1.f;
-        knee_hit = kc;
-        n_knee += kc ? 1.f : 0.f;
-        n_stumble += ((sqrtf(ff[0] * ff[0] + ff[1] * ff[1]) > 5.f) && (fabsf(ff[2]) < 1.f)) ? 1.f : 0.f;
-        const bool contact = ff[2] > 1.f;
-        float fat = fat_b[k];
-        const bool first = (fat > 0.f) && contact;
-        fat += P.dt;
-        air += (fat - 0.5f) * (first ? 1.f : 0.f);
-        fat = contact ? 0.f : fat;
-        if (valid) fat_b[k] = fat;
-    }
-    n_knee = lane_sum<4>(n_knee); n_stumble = lane_sum<4>(n_stumble); air = lane_sum<4>(air);
-    const float any_knee = lane_sum<4>(knee_hit ? 1.f : 0.f);
-
-    // prepare quantities (:464-471)
-    float *cmd = (float *)B.p[B2G_T_COMMANDS] + (size_t)e * 4;
-    const float gvec[3] = {0.f, 0.f, -1.f}, fvec[3] = {1.f, 0.f, 0.f};
-    float blv[3], bav[3], pg[3], fwd[3];
-    t_quat_rotate(rs.rq, rs.rv, blv, -1.f);
-    t_quat_rotate(rs.rq, rs.rw, bav, -1.f);
-    t_quat_rotate(rs.rq, gvec, pg, -1.f);
-    t_quat_apply(rs.rq, fvec, fwd);
-    const float heading = atan2f(fwd[1], fwd[0]);
-    const float c0 = cmd[0], c1 = cmd[1], c3 = cmd[3];
-    const float c2 = fminf(fmaxf(0.5f * t_wrap_to_pi(c3 - heading), -1.f), 1.f);
-
-    // check_termination (:294-300)
-    const float *fb = cf + 3 * P.base_body;
-    bool reset = sqrtf(fb[0] * fb[0] + fb[1] * fb[1] + fb[2] * fb[2]) > 1.f;
-    if (!P.allow_knee_contacts) reset = reset || (any_knee > 0.f);
-    if (progress >= (long long)P.max_episode_length - 1) reset = true;
-
-    float part = 0.f;
-    if (lane == 0 && valid) {
-        // compute_reward (:315-382)
-        const float *R = P.rew_scales;
-        const float ex = c0 - blv[0], ey = c1 - blv[1];
-        const float lin_err = ex * ex + ey * ey;
-        const float ang_err = (c2 - bav[2]) * (c2 - bav[2]);
-        float t[13];
-        t[0] = expf(-lin_err / 0.25f) * R[1];                    // lin_vel_xy
-        t[1] = blv[2] * blv[2] * R[2];                           // lin_vel_z
-        t[2] = expf(-ang_err / 0.25f) * R[3];                    // ang_vel_z
-        t[3] = (bav[0] * bav[0] + bav[1] * bav[1]) * R[4];       // ang_vel_xy
-        t[4] = (pg[0] * pg[0] + pg[1] * pg[1]) * R[5];           // orient
-        t[5] = s_torque * R[6];                                  // torques
-        t[6] = s_jacc * R[7];                                    // joint_acc
-        t[7] = (rs.rp[2] - 0.52f) * (rs.rp[2] - 0.52f) * R[8];   // base_height
-        t[8] = air * R[9] * ((sqrtf(c0 * c0 + c1 * c1) > 0.1f) ? 1.f : 0.f);   // air_time
-        t[9] = n_knee * R[10];                                   // collision
-        t[10] = n_stumble * R[11];                               // stumble
-        t[11] = s_arate * R[12];                                 // action_rate
-        t[12] = s_hip * R[13];                                   // hip
-        float rew = t[0] + t[2] + t[1] + t[3] + t[4] + t[7] + t[5] + t[6] + t[9] + t[11] + t[8] + t[12] + t[10];
-        rew = fmaxf(rew, 0.f);
-        const uint8_t *to = (const uint8_t *)B.p[B2G_T_TIMEOUT];
-        rew += R[0] * (reset ? 1.f : 0.f) * ((to && to[e]) ? 0.f : 1.f);
-        ((float *)B.p[B2G_T_REW])[e] = rew;
-        float *es = (float *)B.p[B2G_T_EPISODE_SUMS];
-#pragma unroll
-        for (int k = 0; k < 13; k++) es[(size_t)k * N + e] += t[k];
-        reset_b[e] = reset ? 1 : 0;
-        progress_b[e] = progress;
-        cmd[2] = c2;
-        float *bs = (float *)B.p[B2G_T_BASE_SCRATCH] + (size_t)e * 12;
-        bs[0] = blv[0]; bs[1] = blv[1]; bs[2] = blv[2]; bs[3] = bav[0]; bs[4] = bav[1]; bs[5] = bav[2];
-        bs[6] = pg[0]; bs[7] = pg[1]; bs[8] = pg[2];
-        if (reset) part = c0 * c0 + c1 * c1;
-    }
-    // deterministic per-block partial of sum over the reset set of |commands_xy|^2
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
-    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = part;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int w = 0; w < BLOCK / 32; w++) tot += s_part[w];
-        float *red = (float *)B.p[B2G_T_REDUCE_SCRATCH];
-        red[blockIdx.x] = tot;
-        if (blockIdx.x == 0) for (int k = 0; k < 16; k++) red[REDUCE_PARTIALS + k] = 0.f;
-    }
+        for (int s = 0; s < NS; s++) {
+            const int d = dofi[s];
+            if (valid) { dw[d] = make_float2(L.q[s], L.qd[s]); if (total > 0 && pd_until > 0) torq[d] = tq[s]; }
+            c.add(P, d, (total > 0 && pd_until > 0) ? tq[s] : torq[d], a_cl[s], L.q[s], L.qd[s], last_a, last_v);
+        }
+        if (valid && lane == 0) store_root((float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
+    });
 }
 
 }  // namespace b2g

@@ -265,4 +265,138 @@ __device__ __forceinline__ void t_quat_apply(const float q[4], const float b[3],
 enum { TAG_PUSH = 1, TAG_RESET = 2, TAG_NOISE = 3 };
 constexpr int REDUCE_PARTIALS = 1024;      // REDUCE_SCRATCH: [0,1024) block partials, then 16 floats of extras sums
 
+// pre_physics_step's PD torque of DOF d from the clamped action a (:443-444)
+__device__ __forceinline__ float anymal_pd_torque(const b2g_anymal_params &P, int d, float a, float q, float qd) {
+    const float t = P.kp * (P.action_scale * a + P.default_dof_pos[d] - q) - P.kd * qd;
+    return fminf(fmaxf(t, -P.torque_limit), P.torque_limit);
+}
+
+// push_robots (:437-439)
+__device__ __forceinline__ void anymal_push(const b2g_anymal_params &P, uint32_t gid, unsigned step_counter, RootState &rs) {
+    if (P.push_robots && P.push_interval > 0 && (step_counter % (unsigned)P.push_interval) == 0) {
+        rs.rv[0] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 0));
+        rs.rv[1] = t_rand_float(-1.f, 1.f, anymal_uniform(P.seed, gid, step_counter, TAG_PUSH, 1));
+    }
+}
+
+// the per-DOF reward sums of compute_reward (:339,342,355,361), from DOF d's last PD torque t, clamped action a and state
+struct AnymalCosts {
+    float torque = 0.f, jacc = 0.f, arate = 0.f, hip = 0.f;
+    __device__ __forceinline__ void add(const b2g_anymal_params &P, int d, float t, float a, float q, float qd,
+                                        const float *last_a, const float *last_v) {
+        torque += t * t;
+        const float dv = last_v[d] - qd; jacc += dv * dv;
+        const float da = last_a[d] - a; arate += da * da;
+        if (d % 3 == 0) hip += fabsf(q - P.default_dof_pos[d]);          // dof_pos[:, [0,3,6,9]]
+    }
+    template <int L> __device__ __forceinline__ void sum_lanes() {
+        torque = lane_sum<L>(torque); jacc = lane_sum<L>(jacc); arate = lane_sum<L>(arate); hip = lane_sum<L>(hip);
+    }
+};
+
+// post_physics_step (:453-475) of AnymalTerrain's first launch, four lanes per env (lane k owns leg k): progress, push,
+// the DOF and root write-back, the contact-force terms, the base quantities, check_termination, compute_reward and its
+// stores, and this block's partial of the norm over the reset set that reset_idx's curriculum needs (:432).
+// write_back(c) is the kernel's own part: it stores the env's DOF states (and, on lane 0, the root) and adds this lane's
+// DOFs to the costs c.  cf: the env's NET_CONTACT rows; s_part: BLOCK / 32 floats of shared memory.
+template <int BLOCK, class WRITE_BACK>
+__device__ __forceinline__ void anymal_post_physics(const b2g_anymal_params &P, const Buffers &B, int N, int e, int lane, bool valid,
+                                                    unsigned step_counter, RootState &rs, const float *cf, float *s_part,
+                                                    WRITE_BACK write_back) {
+    long long *progress_b = (long long *)B.p[B2G_T_PROGRESS];
+    long long *reset_b = (long long *)B.p[B2G_T_RESET];
+    const long long progress = progress_b[e] + 1;
+    const uint32_t gid = (uint32_t)(e + P.env_id_offset);
+    anymal_push(P, gid, step_counter, rs);
+    AnymalCosts c;
+    write_back(c);
+    c.sum_lanes<4>();
+
+    // contact-force terms: every lane looks at bodies base / knee[lane] / foot[lane]
+    float *fat_b = (float *)B.p[B2G_T_FEET_AIR_TIME] + (size_t)e * 4;
+    float n_knee = 0.f, n_stumble = 0.f, air = 0.f;
+    __syncwarp();
+    const float *fk = cf + 3 * P.knee_bodies[lane], *ff = cf + 3 * P.feet_bodies[lane];
+    const bool knee_hit = sqrtf(fk[0] * fk[0] + fk[1] * fk[1] + fk[2] * fk[2]) > 1.f;
+    n_knee += knee_hit ? 1.f : 0.f;
+    n_stumble += ((sqrtf(ff[0] * ff[0] + ff[1] * ff[1]) > 5.f) && (fabsf(ff[2]) < 1.f)) ? 1.f : 0.f;
+    const bool contact = ff[2] > 1.f;
+    float fat = fat_b[lane];
+    const bool first = (fat > 0.f) && contact;
+    fat += P.dt;
+    air += (fat - 0.5f) * (first ? 1.f : 0.f);
+    fat = contact ? 0.f : fat;
+    if (valid) fat_b[lane] = fat;
+    n_knee = lane_sum<4>(n_knee); n_stumble = lane_sum<4>(n_stumble); air = lane_sum<4>(air);
+    const float any_knee = lane_sum<4>(knee_hit ? 1.f : 0.f);
+
+    // prepare quantities (:464-471)
+    float *cmd = (float *)B.p[B2G_T_COMMANDS] + (size_t)e * 4;
+    const float gvec[3] = {0.f, 0.f, -1.f}, fvec[3] = {1.f, 0.f, 0.f};
+    float blv[3], bav[3], pg[3], fwd[3];
+    t_quat_rotate(rs.rq, rs.rv, blv, -1.f);
+    t_quat_rotate(rs.rq, rs.rw, bav, -1.f);
+    t_quat_rotate(rs.rq, gvec, pg, -1.f);
+    t_quat_apply(rs.rq, fvec, fwd);
+    const float heading = atan2f(fwd[1], fwd[0]);
+    const float c0 = cmd[0], c1 = cmd[1], c3 = cmd[3];
+    const float c2 = fminf(fmaxf(0.5f * t_wrap_to_pi(c3 - heading), -1.f), 1.f);
+
+    // check_termination (:294-300)
+    const float *fb = cf + 3 * P.base_body;
+    bool reset = sqrtf(fb[0] * fb[0] + fb[1] * fb[1] + fb[2] * fb[2]) > 1.f;
+    if (!P.allow_knee_contacts) reset = reset || (any_knee > 0.f);
+    if (progress >= (long long)P.max_episode_length - 1) reset = true;
+
+    float part = 0.f;
+    if (lane == 0 && valid) {
+        // compute_reward (:315-382)
+        const float *R = P.rew_scales;
+        const float ex = c0 - blv[0], ey = c1 - blv[1];
+        const float lin_err = ex * ex + ey * ey;
+        const float ang_err = (c2 - bav[2]) * (c2 - bav[2]);
+        float t[13];
+        t[0] = expf(-lin_err / 0.25f) * R[1];                    // lin_vel_xy
+        t[1] = blv[2] * blv[2] * R[2];                           // lin_vel_z
+        t[2] = expf(-ang_err / 0.25f) * R[3];                    // ang_vel_z
+        t[3] = (bav[0] * bav[0] + bav[1] * bav[1]) * R[4];       // ang_vel_xy
+        t[4] = (pg[0] * pg[0] + pg[1] * pg[1]) * R[5];           // orient
+        t[5] = c.torque * R[6];                                  // torques
+        t[6] = c.jacc * R[7];                                    // joint_acc
+        t[7] = (rs.rp[2] - 0.52f) * (rs.rp[2] - 0.52f) * R[8];   // base_height
+        t[8] = air * R[9] * ((sqrtf(c0 * c0 + c1 * c1) > 0.1f) ? 1.f : 0.f);   // air_time
+        t[9] = n_knee * R[10];                                   // collision
+        t[10] = n_stumble * R[11];                               // stumble
+        t[11] = c.arate * R[12];                                 // action_rate
+        t[12] = c.hip * R[13];                                   // hip
+        float rew = t[0] + t[2] + t[1] + t[3] + t[4] + t[7] + t[5] + t[6] + t[9] + t[11] + t[8] + t[12] + t[10];
+        rew = fmaxf(rew, 0.f);
+        const uint8_t *to = (const uint8_t *)B.p[B2G_T_TIMEOUT];
+        rew += R[0] * (reset ? 1.f : 0.f) * ((to && to[e]) ? 0.f : 1.f);
+        ((float *)B.p[B2G_T_REW])[e] = rew;
+        float *es = (float *)B.p[B2G_T_EPISODE_SUMS];
+#pragma unroll
+        for (int k = 0; k < 13; k++) es[(size_t)k * N + e] += t[k];
+        reset_b[e] = reset ? 1 : 0;
+        progress_b[e] = progress;
+        cmd[2] = c2;
+        float *bs = (float *)B.p[B2G_T_BASE_SCRATCH] + (size_t)e * 12;
+        bs[0] = blv[0]; bs[1] = blv[1]; bs[2] = blv[2]; bs[3] = bav[0]; bs[4] = bav[1]; bs[5] = bav[2];
+        bs[6] = pg[0]; bs[7] = pg[1]; bs[8] = pg[2];
+        if (reset) part = c0 * c0 + c1 * c1;
+    }
+    // deterministic per-block partial of sum over the reset set of |commands_xy|^2
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = part;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float tot = 0.f;
+        for (int w = 0; w < BLOCK / 32; w++) tot += s_part[w];
+        float *red = (float *)B.p[B2G_T_REDUCE_SCRATCH];
+        red[blockIdx.x] = tot;
+        if (blockIdx.x == 0) for (int k = 0; k < 16; k++) red[REDUCE_PARTIALS + k] = 0.f;
+    }
+}
+
 }  // namespace b2g
