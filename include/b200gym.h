@@ -193,8 +193,8 @@ enum {
     B2G_T_OBJ_FORCE = 46,      /* f32 (N,3) */
     B2G_T_RANDOM_FORCE_PROB = 47, /* f32 (N)   random_force_prob, shadow_hand.py:198,642 */
     /* physical domain randomisation of a sim with a free object (ShadowHand's actor_params.object, tendon_properties and
-     * sim_params.gravity, vec_task.py:722-828).  NULL = the model's own values; b2g_bind refuses them (B2G_E_UNSUPPORTED) on a
-     * sim without a free object.  Any per-env parameter bound on such a sim (these three or ENV_MASS_SCALE / ENV_DOF_PROPS /
+     * sim_params.gravity, vec_task.py:722-828).  NULL = the model's own values; b2g_bind refuses ENV_OBJ_PROPS and
+     * ENV_TENDON_DAMPING (B2G_E_UNSUPPORTED) on a sim without a free object.  Any per-env parameter bound on such a sim (these three or ENV_MASS_SCALE / ENV_DOF_PROPS /
      * ENV_FRICTION) selects the randomised instantiation of its simulate and ShadowHand step kernels.  Frictions combine as
      * PhysX's default, the average of the two materials: ENV_FRICTION (the articulation's shapes) with the ground and with the
      * object, the object's with the ground; where only one of ENV_FRICTION / ENV_OBJ_PROPS is bound, obj_mu stands in for the
@@ -203,7 +203,13 @@ enum {
                                   inertia x s^2), mass factor (mass, inertia and the contact gains obj_kn / obj_cn, which are
                                   proportional to the mass), friction, unused */
     B2G_T_ENV_TENDON_DAMPING = 49, /* f32 (N,nten)  damping of each tendon (ten_d) */
-    B2G_T_GRAVITY = 50,        /* f32 (3)    the sim's gravity, read on the device by every sub-step (bodies with gravity on) */
+    /* f32 (3)  the sim's gravity (bodies with gravity on), read on the device by every sub-step of the kernels that take it: the
+     * randomised simulate and ShadowHand step of a free-object sim, and the Humanoid step at its 4 lanes and 64 threads with
+     * device or staged I/O (with or without link-link contact).  Bound on any sim; every other physics launch -- b2g_simulate
+     * without a free object, the Ant, Cartpole and AnymalTerrain steps, the four-chain kernels, a Humanoid combination without
+     * the instantiation -- fails with B2G_E_UNSUPPORTED while it is bound.  Resets, body state and the kinematic tensors
+     * involve no gravity and ignore it. */
+    B2G_T_GRAVITY = 50,
     B2G_T_COUNT = 51
 };
 

@@ -41,12 +41,12 @@ def _num_envs(root, default):
     return default if root["num_envs"] in ("", None) else int(root["num_envs"])
 
 
-# cfg/task/ShadowHand.yaml randomization_params (the same block as ShadowHandOpenAI_FF.yaml / ShadowHandTest.yaml): what
-# task.randomize=True turns on
+# the reference's randomization_params blocks: what task.randomize=True turns on
 def _dr(lo, hi, op, dist, **kw):
     return {"range": [lo, hi], "operation": op, "distribution": dist, **kw}
 
 
+# cfg/task/ShadowHand.yaml (the same block as ShadowHandOpenAI_FF.yaml / ShadowHandTest.yaml)
 _SHADOW_HAND_DR = {
     "frequency": 720,
     "observations": _dr(0, .002, "additive", "gaussian", range_correlated=[0, .001]),
@@ -64,6 +64,36 @@ _SHADOW_HAND_DR = {
         "object": {"scale": _dr(0.95, 1.05, "scaling", "uniform", setup_only=True),
                    "rigid_body_properties": {"mass": _dr(0.5, 1.5, "scaling", "uniform", setup_only=True)},
                    "rigid_shape_properties": {"friction": _dr(0.7, 1.3, "scaling", "uniform", num_buckets=250)}}}}
+
+
+# cfg/task/Ant.yaml and cfg/task/Humanoid.yaml randomization_params
+_ANT_DR = {
+    "frequency": 600,
+    "observations": _dr(0, .002, "additive", "gaussian"),
+    "actions": _dr(0., .02, "additive", "gaussian"),
+    "actor_params": {
+        "ant": {"color": True,
+                "rigid_body_properties": {"mass": _dr(0.5, 1.5, "scaling", "uniform", setup_only=True)},
+                "dof_properties": {"damping": _dr(0.5, 1.5, "scaling", "uniform"), "stiffness": _dr(0.5, 1.5, "scaling", "uniform"),
+                                   "lower": _dr(0, 0.01, "additive", "gaussian"), "upper": _dr(0, 0.01, "additive", "gaussian")}}}}
+
+
+def _lin(lo, hi, op, dist, **kw):          # Humanoid.yaml's entries ramp in over 3000 frames
+    return _dr(lo, hi, op, dist, **kw, schedule="linear", schedule_steps=3000)
+
+
+_HUMANOID_DR = {
+    "frequency": 600,
+    "observations": _dr(0, .002, "additive", "gaussian"),
+    "actions": _dr(0., .02, "additive", "gaussian"),
+    "sim_params": {"gravity": _lin(0, 0.4, "additive", "gaussian")},
+    "actor_params": {
+        "humanoid": {"color": True,
+                     "rigid_body_properties": {"mass": _lin(0.5, 1.5, "scaling", "uniform", setup_only=True)},
+                     "rigid_shape_properties": {"friction": _lin(0.7, 1.3, "scaling", "uniform", num_buckets=500),
+                                                "restitution": _lin(0., 0.7, "scaling", "uniform")},
+                     "dof_properties": {"damping": _lin(0.5, 1.5, "scaling", "uniform"), "stiffness": _lin(0.5, 1.5, "scaling", "uniform"),
+                                        "lower": _lin(0, 0.01, "additive", "gaussian"), "upper": _lin(0, 0.01, "additive", "gaussian")}}}}
 
 
 def _builtin_task(name, root):
@@ -87,7 +117,7 @@ def _builtin_task(name, root):
                         "deathCost": -2.0, "terminationHeight": 0.31, "plane": plane,
                         "asset": {"assetFileName": "mjcf/nv_ant.xml"}, "enableCameraSensors": False},
                 "sim": _sim(root, _physx(root)),
-                "task": {"randomize": False, "randomization_params": {}}}
+                "task": {"randomize": False, "randomization_params": copy.deepcopy(_ANT_DR)}}
     if name == "Humanoid":
         return {"name": "Humanoid", "physics_engine": root["physics_engine"],
                 "env": {"numEnvs": _num_envs(root, 4096), "envSpacing": 5, "episodeLength": 1000,
@@ -97,7 +127,7 @@ def _builtin_task(name, root):
                         "jointsAtLimitCost": 0.25, "deathCost": -1.0, "terminationHeight": 0.8, "plane": plane,
                         "asset": {"assetFileName": "mjcf/nv_humanoid.xml"}, "enableCameraSensors": False},
                 "sim": _sim(root, _physx(root)),
-                "task": {"randomize": False, "randomization_params": {}}}
+                "task": {"randomize": False, "randomization_params": copy.deepcopy(_HUMANOID_DR)}}
     if name == "ShadowHand":
         sim = _sim(root, _physx(root, num_position_iterations=8, contact_offset=0.002, max_depenetration_velocity=1000.0))
         sim.update({"dt": 0.01667, "substeps": 2})

@@ -197,7 +197,9 @@ __global__ void __launch_bounds__(BLOCK) simulate_kernel(const DevModel *__restr
 #define B2G_MINBLOCKS 4
 #endif
 
-template <int L, bool HF, bool HUM, int BLOCK, bool TILES, bool HOSTIO = false, bool SELF = false>
+// DR: the sub-steps read a bound gravity vector (B2G_T_GRAVITY; the Humanoid's sim_params.gravity randomisation), a separate
+// instantiation chosen at run time when the tensor is bound
+template <int L, bool HF, bool HUM, int BLOCK, bool TILES, bool HOSTIO = false, bool SELF = false, bool DR = false>
 __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK == 64 && !HUM ? 2 * B2G_MINBLOCKS : 1))) loco_step_kernel(
     const DevModel *__restrict__ gm, const int16_t *__restrict__ hf, Buffers B, const __grid_constant__ b2g_task_params P,
     const float *__restrict__ actions_in, int N, TileArgs ta) {
@@ -259,16 +261,17 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     mbar_wait(&mbar, 0);
     if (tiles) mbar_wait(&mbar2, 0);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");       // the next step's grid may begin its own prologue
-    using ST = Stepper<L, HF, BLOCK, false, SELF>;
+    using ST = Stepper<L, HF, BLOCK, false, SELF, DR>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;
     const bool valid = env < N;
     const int e = valid ? env : N - 1;
     const int el = e - env0;                             // env index inside this block's tiles
     const int NS = sm.ns;
-    ST st = make_stepper<L, HF, BLOCK, false, SELF>(&sm, hf, lane);
+    ST st = make_stepper<L, HF, BLOCK, false, SELF, DR>(&sm, hf, lane);
     st.gmodel = gm;
     attach_env_params_generic(st, sm, B, e);
+    if (DR) st.dr_grav = (const float *)B.p[B2G_T_GRAVITY];
     {
         const char *pk = reinterpret_cast<const char *>(&sm) + offsetof(DevModel, slots) + (size_t)sm.ns * MAX_LANES * sizeof(SlotRec);
         st.links = reinterpret_cast<const LinkC *>(pk);
@@ -695,8 +698,8 @@ extern "C" int b2g_bind(b2g_sim *s, int32_t slot, void *ptr, size_t bytes) {
         default: need = 0; break;   // ACTIONS / OBS / OBS_CLIPPED are checked against the task in b2g_set_task
     }
     if (ptr && bytes < need) return fail(B2G_E_INVALID, "b2g_bind: buffer smaller than the tensor's layout requires");
-    if ((slot == B2G_T_ENV_OBJ_PROPS || slot == B2G_T_ENV_TENDON_DAMPING || slot == B2G_T_GRAVITY) && !s->hm.obj_on)
-        return fail(B2G_E_UNSUPPORTED, "b2g_bind: object, tendon and gravity parameters need a sim with a free object");
+    if ((slot == B2G_T_ENV_OBJ_PROPS || slot == B2G_T_ENV_TENDON_DAMPING) && !s->hm.obj_on)
+        return fail(B2G_E_UNSUPPORTED, "b2g_bind: object and tendon parameters need a sim with a free object");
     s->buf.p[slot] = ptr; s->buf_bytes[slot] = bytes;
     return B2G_OK;
 }
@@ -704,6 +707,14 @@ extern "C" int b2g_bind(b2g_sim *s, int32_t slot, void *ptr, size_t bytes) {
 static int require(const b2g_sim *s, std::initializer_list<int> slots, const char *who) {
     for (int k : slots) if (!s->buf.p[k]) return fail(B2G_E_UNBOUND, std::string(who) + ": tensor slot " + std::to_string(k) + " is not bound");
     return B2G_OK;
+}
+
+// A bound gravity vector (B2G_T_GRAVITY) is read by the free-object DR kernels and the Humanoid's gravity instantiations
+// only: every other physics launch refuses it rather than step under the model's gravity
+static int refuse_gravity(const b2g_sim *s, const std::string &who) {
+    if (!s->buf.p[B2G_T_GRAVITY]) return B2G_OK;
+    return fail(B2G_E_UNSUPPORTED, who + ": no kernel of this combination reads a bound GRAVITY vector; unbind it or use a sim whose "
+                                         "kernels read it (a free object, or the Humanoid task)");
 }
 
 // the action and observation counts of the task set on the sim
@@ -837,6 +848,7 @@ extern "C" int b2g_simulate(b2g_sim *s, void *stream) {
     CUDA_TRY(cudaSetDevice(s->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int N = s->num_envs;
+    if (!s->hm.obj_on) { rc = refuse_gravity(s, "b2g_simulate(sim without a free object)"); if (rc) return rc; }
     if (s->quad_ns) {
         const bool self = s->hm.self_on != 0;
         const size_t dyn = ((size_t)quad_park_f4(s->quad_ns, self) * QUAD_SIM_BLOCK + quad_model_f4(s->quad_ns, self)) * sizeof(float4);
@@ -1030,6 +1042,7 @@ static int anymal_step(b2g_sim *s, const float *actions, void *stream) {
                      "b2g_task_step(AnymalTerrain)");
     if (rc) return rc;
     if (P.custom_origins) { rc = require(s, {B2G_T_ENV_ORIGINS, B2G_T_TERRAIN_LEVELS, B2G_T_TERRAIN_TYPES, B2G_T_TERRAIN_ORIGINS}, "b2g_task_step(AnymalTerrain)"); if (rc) return rc; }
+    rc = refuse_gravity(s, "b2g_task_step(AnymalTerrain)"); if (rc) return rc;
     CUDA_TRY(cudaSetDevice(s->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int N = s->num_envs, grid = (N * 4 + 127) / 128;
@@ -1065,7 +1078,8 @@ constexpr int QUAD_LOCO_BLOCK = 64;
 using QuadLocoKernel = void (*)(const float4 *, Buffers, b2g_task_params, const float *, int, int, TileArgs);
 using LocoKernel = void (*)(const DevModel *, const int16_t *, Buffers, b2g_task_params, const float *, int, TileArgs);
 static QuadLocoKernel quad_loco_kernel_for(int spec, bool hostio, bool lean);
-static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self);
+static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self, bool grav);
+static LocoKernel loco_gravity_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self);
 
 // One VecTask.step(); io: the pinned host buffers the Ant / Humanoid step kernel writes to itself (null: device I/O)
 static int task_step(b2g_sim *s, const float *actions, void *stream, const HostOut *io) {
@@ -1083,11 +1097,13 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
     cudaStream_t st = (cudaStream_t)stream;
     const int blk = s->block, grid = ((int)N * s->lanes + blk - 1) / blk;
     if (P.task == B2G_TASK_CARTPOLE) {
+        rc = refuse_gravity(s, "b2g_task_step(Cartpole)"); if (rc) return rc;
         if (blk != 128) return fail(B2G_E_UNSUPPORTED, "cartpole: unexpected CTA size");
         return launch(s, cartpole_step_kernel<128>, grid, blk, s->dyn_smem, st, SMEM, s->dm, s->buf, P, actions, (int)N);
     }
     rc = require(s, {B2G_T_POTENTIALS, B2G_T_PREV_POTENTIALS, B2G_T_INITIAL_ROOT}, "b2g_task_step"); if (rc) return rc;
-    const bool hum = P.task == B2G_TASK_HUMANOID;
+    const bool hum = P.task == B2G_TASK_HUMANOID, grav = s->buf.p[B2G_T_GRAVITY] != nullptr;
+    if (!hum) { rc = refuse_gravity(s, "b2g_task_step(Ant)"); if (rc) return rc; }
     const int O = P.num_obs, ns6 = 6 * s->hm.nsens;
     const bool clip_sep = s->buf.p[B2G_T_OBS_CLIPPED] && s->buf.p[B2G_T_OBS_CLIPPED] != s->buf.p[B2G_T_OBS];
     if (!hum && s->quad_ns == 2 && !s->d_hf) {           // Ant on the quad sub-step (whole tiles only)
@@ -1113,8 +1129,13 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
                                (((size_t)s->hm.ncp * sizeof(CpC) + 15) & ~(size_t)15);
     const size_t io_used = tiles ? io_bytes : 16;
     const size_t dyn = state_bytes + io_used + model_bytes;
-    const LocoKernel k = loco_kernel_for(s->lanes, blk, hum, tiles, io != nullptr, s->hm.self_on);
-    if (!k) return fail(B2G_E_UNSUPPORTED, "no locomotion step kernel instantiated for this (lanes, CTA size, task, tiles, host I/O, self-collision) combination");
+    const LocoKernel k = loco_kernel_for(s->lanes, blk, hum, tiles, io != nullptr, s->hm.self_on, grav);
+    if (!k) {
+        char what[160];
+        snprintf(what, sizeof(what), "(lanes %d, CTA size %d, %s, tiles %d, host I/O %d, self-collision %d, gravity bound %d)", s->lanes, blk,
+                 hum ? "Humanoid" : "Ant", (int)tiles, (int)(io != nullptr), (int)(s->hm.self_on != 0), (int)grav);
+        return fail(B2G_E_UNSUPPORTED, std::string("no locomotion step kernel instantiated for this combination ") + what);
+    }
     return launch(s, k, grid, blk, dyn, st, SMEM_PDL, (const DevModel *)s->dm, (const int16_t *)s->d_hf, s->buf, P, actions, (int)N,
                   tile_args(tiles, state_bytes, state_bytes + io_used, actions, io));
 }
@@ -1130,9 +1151,11 @@ static QuadLocoKernel quad_loco_kernel_for(int spec, bool hostio, bool lean) {
 }
 
 // the fused Ant / Humanoid step on the generic Stepper (ground plane): (lanes, CTA size, Humanoid, tiles, host I/O,
-// self-collision).  Host I/O needs the tiles; self-collision runs 4-lane Humanoid-type tasks with device or staged I/O.
-static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self) {
+// self-collision, gravity bound).  Host I/O needs the tiles; self-collision runs 4-lane Humanoid-type tasks with device or
+// staged I/O.
+static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self, bool grav) {
     if (hostio && !tiles) return nullptr;
+    if (grav) return loco_gravity_kernel_for(lanes, block, hum, tiles, hostio, self);
     if (self) {
         if (!hum || lanes != 4 || hostio) return nullptr;
         if (block == 64) return tiles ? loco_step_kernel<4, false, true, 64, true, false, true> : loco_step_kernel<4, false, true, 64, false, false, true>;
@@ -1162,6 +1185,14 @@ static LocoKernel loco_kernel_for(int lanes, int block, bool hum, bool tiles, bo
     return nullptr;
 }
 
+// the Humanoid step reading a bound gravity vector: the Humanoid's own 4 lanes and 64 threads, with and without link-link
+// contact (the reference's collision filter 0), device or staged I/O
+static LocoKernel loco_gravity_kernel_for(int lanes, int block, bool hum, bool tiles, bool hostio, bool self) {
+    if (!hum || hostio || key(lanes, block) != key(4, 64)) return nullptr;
+    if (self) return tiles ? loco_step_kernel<4, false, true, 64, true, false, true, true> : loco_step_kernel<4, false, true, 64, false, false, true, true>;
+    return tiles ? loco_step_kernel<4, false, true, 64, true, false, false, true> : loco_step_kernel<4, false, true, 64, false, false, false, true>;
+}
+
 extern "C" int b2g_task_step(b2g_sim *s, const float *actions, void *stream) { return task_step(s, actions, stream, nullptr); }
 
 // K x VecTask.step() with the actions of all K steps given up front (open-loop / random-action rollouts)
@@ -1171,7 +1202,8 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     if (!s->has_task && !s->has_anymal && !s->has_hand) return fail(B2G_E_INVALID, "b2g_task_rollout: call b2g_set_task first");
     const size_t N = s->num_envs;
     constexpr int QB = 64, EPB = 16;
-    const bool fused = s->has_task && s->task.task == B2G_TASK_ANT && s->quad_ns == 2 && !s->d_hf && whole_tiles(N, EPB);
+    // (a bound gravity vector takes the single-step path, whose Ant step refuses it)
+    const bool fused = s->has_task && s->task.task == B2G_TASK_ANT && s->quad_ns == 2 && !s->d_hf && whole_tiles(N, EPB) && !s->buf.p[B2G_T_GRAVITY];
     cudaStream_t st = (cudaStream_t)stream;
     if (!fused) {
         // every other task / shape: K single steps, their results copied into the (K, N, .) outputs (same semantics, no fusion)

@@ -48,7 +48,7 @@ class _Locomotion(VecTask):
         self.plane_static_friction = e["plane"]["staticFriction"]
         self.plane_dynamic_friction = e["plane"]["dynamicFriction"]
         self.plane_restitution = e["plane"]["restitution"]
-        # randomize: observation / action noise is applied by the base class; physical randomisation raises there
+        # randomize: the base class applies the noise and binds the per-env physical parameters (and the Humanoid's gravity)
         cfg["env"]["numObservations"] = self.NUM_OBS
         cfg["env"]["numActions"] = self.NUM_ACT
         self.up_axis_idx = 2
@@ -166,6 +166,13 @@ class Ant(_Locomotion):
 class Humanoid(_Locomotion):
     HUMANOID = True
     NUM_OBS, NUM_ACT, START_HEIGHT, DEFAULT_ASSET, ALIVE = 108, 21, 1.34, "mjcf/nv_humanoid.xml", 2.0
+
+    # domain randomisation (task.randomize): the Humanoid step kernels read a bound gravity vector
+    dr_gravity = True
+
+    def _randomize_this_step(self):
+        # humanoid.py:255-256: apply_randomizations runs inside reset_idx, on steps where some env resets
+        return bool(self.reset_buf.any())
 
     def _fill_extras(self):
         pass

@@ -6,9 +6,10 @@
   reads (include/b200gym.h B2G_T_ENV_MASS_SCALE / ENV_DOF_PROPS / ENV_FRICTION), refreshed on the device for the envs
   that are about to reset and whose randomisation counter passed `frequency` -- the reference's selection rule
   (vec_task.py:631-637).  Supported: rigid_body_properties.mass, dof_properties.{damping, stiffness, lower, upper},
-  rigid_shape_properties.friction, and for a sim with a free object (ShadowHand: actors `hand` and `object`)
-  tendon_properties, the object's scale, mass and friction (B2G_T_ENV_OBJ_PROPS / ENV_TENDON_DAMPING) and
-  sim_params.gravity (B2G_T_GRAVITY); anything else raises.
+  rigid_shape_properties.{friction, restitution (scaled, no effect)}, sim_params.gravity (B2G_T_GRAVITY) for the tasks whose
+  kernels read it (ShadowHand, Humanoid), and for a sim with a free object (ShadowHand: actors `hand` and `object`)
+  tendon_properties and the object's scale, mass and friction (B2G_T_ENV_OBJ_PROPS / ENV_TENDON_DAMPING); anything else
+  raises.
 
 A NoiseModel is built from one YAML entry
 
@@ -146,14 +147,17 @@ class PhysicalRandomizer:
     actor type, the articulation.
 
     articulation: rigid_body_properties.mass, dof_properties.{damping, stiffness, lower, upper} (a position-driven DOF's damping
-    is all of its velocity damping and its stiffness the drive's kp, as get_actor_dof_properties reports them), rigid_shape_properties.friction, and
-    with tendons tendon_properties.{damping, stiffness}: the damping of each tendon; the active tendons' spring stiffness is 0
-    in the reference (shadow_hand.py:255-266), so scaling it changes nothing and it is drawn but not applied.
+    is all of its velocity damping and its stiffness the drive's kp, as get_actor_dof_properties reports them),
+    rigid_shape_properties.{friction, restitution}, and with tendons tendon_properties.{damping, stiffness}: the damping of
+    each tendon; the active tendons' spring stiffness is 0 in the reference (shadow_hand.py:255-266), so scaling it changes
+    nothing and it is drawn but not applied.  Restitution likewise: the MJCF shapes carry none (0), so under `scaling` it stays
+    0 and is drawn but not applied (the contact model has no restitution); `additive` raises, as it would give the shapes a
+    restitution the kernels do not model.
     object: scale (contact extents x s, inertia x s^2, mass unchanged: a modelling choice), rigid_body_properties.mass (mass,
     inertia and contact gains), rigid_shape_properties.friction.
     Friction is one value per env and actor (the reference draws one per shape); `num_buckets` rounds it onto the bucket grid."""
     SUPPORTED = {"rigid_body_properties": ("mass",), "dof_properties": ("damping", "stiffness", "lower", "upper"),
-                 "rigid_shape_properties": ("friction",)}
+                 "rigid_shape_properties": ("friction", "restitution")}
     OBJECT_SUPPORTED = {"rigid_body_properties": ("mass",), "rigid_shape_properties": ("friction",)}
 
     def __init__(self, actor_params, model, num_envs, device, frequency, actors=None, obj=None, tendon_damping=None):
@@ -179,6 +183,9 @@ class PhysicalRandomizer:
                 for attr in attrs:
                     if attr not in supported[group]:
                         raise NotImplementedError(f"actor_params.{name}.{group}.{attr} is not provided")
+                    if attr == "restitution" and attrs[attr]["operation"] != "scaling":
+                        raise NotImplementedError(f"actor_params.{name}.{group}.restitution: scaling only (the shapes' restitution "
+                                                  "is 0 and the contact model has none)")
             self.entries.append((name, role, props))
         art = [p for _, r, p in self.entries if r == "articulation"]
         ob = [p for _, r, p in self.entries if r == "object"]
@@ -273,6 +280,8 @@ class PhysicalRandomizer:
             if attr == "damping":
                 new = og[None] * smp if scaling else og[None] + smp
                 self.tendon_damping.copy_(torch.where(mask[:, None], new, self.tendon_damping))
+        elif attr == "restitution":                                  # a scaled 0: drawn, nothing to apply
+            _sample(entry, (N,), frame, self.device)
         else:                                                        # friction: one value per env (all its shapes)
             smp = _sample(entry, (N,), frame, self.device)
             new = self.og_friction * smp if scaling else self.og_friction + smp

@@ -80,6 +80,7 @@ def main(argv=None):
     ap.add_argument("--mini-epochs", type=int, default=4)      # HumanoidPPO.yaml: 5
     ap.add_argument("--critic-coef", type=float, default=2.0)  # HumanoidPPO.yaml: 4
     ap.add_argument("--self-collision", action="store_true")   # Humanoid, AnymalTerrain: env.selfCollision=True
+    ap.add_argument("--randomize", action="store_true")        # task.randomize=True: the task's randomization_params block
     ap.add_argument("--kl-threshold", type=float, default=0.008)   # ShadowHandPPO.yaml: 0.016
     ap.add_argument("--reward-scale", type=float, default=0.01)    # reward_shaper.scale_value; CartpolePPO.yaml 0.1, AnymalTerrainPPO.yaml 1.0
     ap.add_argument("--bounds-coef", type=float, default=1e-4)     # bounds_loss_coef; AnymalTerrainPPO.yaml 0
@@ -92,6 +93,10 @@ def main(argv=None):
     if args.self_collision:
         from isaacgymenvs_b200 import config
         cfg = config.builtin_cfg(args.task, {"sim_device": dev, "rl_device": dev}); cfg["task"]["env"]["selfCollision"] = True
+    if args.randomize:
+        from isaacgymenvs_b200 import config
+        cfg = cfg or config.builtin_cfg(args.task, {"sim_device": dev, "rl_device": dev})
+        cfg["task"]["task"]["randomize"] = True
     if args.env:
         from isaacgymenvs_b200 import config
         cfg = cfg or config.builtin_cfg(args.task, {"sim_device": dev, "rl_device": dev})

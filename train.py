@@ -9,6 +9,7 @@ bounds loss) and runs the compact learner of tools/train_ppo.py, which drives th
     python train.py task=Ant headless=True                       # 4096 envs, 500 epochs (AntPPO.yaml)
     python train.py task=ShadowHand num_envs=8192 max_iterations=300 task.env.objectType=pen task.env.forceScale=1.0
     python train.py task=Humanoid seed=7 sim_device=cuda:0 rl_device=cuda:0 task.env.selfCollision=True
+    python train.py task=Humanoid task.task.randomize=True       # the randomization_params block of Humanoid.yaml
 
 Demonstration tooling (DESIGN.md section 6e), not part of the measured hot path.
 """
@@ -48,9 +49,13 @@ def to_ppo_argv(ov):
     hp = PPO[task]
     known = {"task", "num_envs", "seed", "max_iterations", "sim_device", "rl_device", "headless", "pipeline", "graphics_device_id",
              "experiment", "wandb_activate", "capture_video", "force_render", "test", "checkpoint", "multi_gpu"}
-    bad = [k for k in ov if k not in known and not k.startswith("task.env.")]
+    bad = [k for k in ov if k not in known and not k.startswith("task.env.") and k != "task.task.randomize"]
     if bad:
-        raise SystemExit(f"train.py: overrides {bad} are not provided here (top-level keys of cfg/config.yaml and task.env.* are)")
+        raise SystemExit(f"train.py: overrides {bad} are not provided here (top-level keys of cfg/config.yaml, task.env.* and "
+                         "task.task.randomize are)")
+    randomize = ov.get("task.task.randomize", "False")
+    if randomize not in ("True", "true", "False", "false"):
+        raise SystemExit(f"train.py: task.task.randomize={randomize!r}: True or False")
     for k in ("test", "checkpoint", "multi_gpu", "capture_video"):
         if ov.get(k, "False") not in ("False", "false", "", "0"):
             raise SystemExit(f"train.py: {k} is not provided by the demonstration learner")
@@ -65,6 +70,8 @@ def to_ppo_argv(ov):
             "--reward-scale", repr(hp["rew_scale"]), "--bounds-coef", repr(hp["bounds"])]
     if selfc:
         argv.append("--self-collision")
+    if randomize in ("True", "true"):
+        argv.append("--randomize")
     if env:
         argv += ["--env", ",".join(f"{k}={v}" for k, v in env.items())]
     if ov.get("experiment"):
