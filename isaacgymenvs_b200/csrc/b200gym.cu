@@ -468,8 +468,7 @@ __global__ void __launch_bounds__(BLOCK) cartpole_step_kernel(const DevModel *__
         int *rc = (int *)B.p[B2G_T_RESET_COUNT];
         const uint32_t count = (uint32_t)rc[e], gid = (uint32_t)(e + P.env_id_offset);
 #pragma unroll
-        for (int s = 0; s < 2; s++)
-            st.set_q(s, 0.2f * (reset_uniform(P.seed, gid, count, s) - 0.5f), 0.5f * (reset_uniform(P.seed, gid, count, 2 + s) - 0.5f));
+        for (int s = 0; s < 2; s++) { const float2 qv = cartpole_reset_dof(P, gid, count, s); st.set_q(s, qv.x, qv.y); }
         progress = 0;
         if (valid) rc[e] = (int)(count + 1);
     }

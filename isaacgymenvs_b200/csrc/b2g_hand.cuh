@@ -45,14 +45,51 @@ __device__ __forceinline__ void t_randomize_rotation_pen(float rand0, float q[4]
     t_quat_axis(rand0 * 3.1415927f, 2, qz);
     t_quat_mul(qx, qz, q);
 }
-// the object's orientation at reset_idx (:625-629)
-__device__ __forceinline__ void t_object_reset_rotation(const b2g_hand_params &P, float rand0, float rand1, float q[4]) {
-    if (P.object_is_pen) t_randomize_rotation_pen(rand0, q);
-    else t_randomize_rotation(rand0, rand1, q);
-}
 // torch_rand_float(-1, 1): (upper - lower) * rand + lower
 __device__ __forceinline__ float hand_rand(uint64_t seed, uint32_t gid, uint32_t count, int idx) {
     return 2.0f * reset_uniform(seed, gid, count, idx) + (-1.0f);
+}
+
+// ---- reset_idx (:612-659), reset_target_pose (:594-610): shared by the fused step and reset_done (b2g_reset.cuh).  Reset
+// stream of reset number `count`, by index: object position 0-2, rotation 3-4 (:625-629); DOF d's position 5 + d (also its
+// target), velocity 5 + nd + d; goal rotation 2 nd + 5, 2 nd + 6; random_force_prob 2 nd + 7.  A goal-only reset
+// draws 0, 1 of stream *goal_count | 2^31.  write: store goal_states, the goal's root row (rows + 26), the new goal_count.
+__device__ __forceinline__ void hand_reset_goal(const b2g_hand_params &P, uint32_t gid, uint32_t count, int nd, bool goal_only,
+                                                int *goal_count, const float *init_rows, float *goal_row, float *rows,
+                                                bool write, float goal_pos[3], float goal_rot[4]) {
+    float r0, r1;
+    if (!goal_only) { r0 = hand_rand(P.seed, gid, count, 2 * nd + 5); r1 = hand_rand(P.seed, gid, count, 2 * nd + 6); }
+    else {
+        const uint32_t gc = (uint32_t)*goal_count | 0x80000000u;
+        r0 = hand_rand(P.seed, gid, gc, 0); r1 = hand_rand(P.seed, gid, gc, 1);
+        if (write) *goal_count = (int)(((uint32_t)*goal_count + 1u) & 0x7fffffffu);
+    }
+    t_randomize_rotation(r0, r1, goal_rot);
+#pragma unroll
+    for (int c = 0; c < 3; c++) goal_pos[c] = init_rows[26 + c];
+    if (write) {
+#pragma unroll
+        for (int c = 0; c < 3; c++) { goal_row[c] = goal_pos[c]; rows[26 + c] = goal_pos[c] + P.goal_displacement[c]; }
+#pragma unroll
+        for (int c = 0; c < 4; c++) { goal_row[3 + c] = goal_rot[c]; rows[29 + c] = goal_rot[c]; }
+#pragma unroll
+        for (int c = 7; c < 13; c++) rows[26 + c] = 0.f;
+    }
+}
+__device__ __forceinline__ void hand_reset_obj(const b2g_hand_params &P, uint32_t gid, uint32_t count, const float *init_rows, ObjState &ob) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) ob.p[c] = init_rows[13 + c] + P.reset_position_noise * hand_rand(P.seed, gid, count, c);
+    const float r3 = hand_rand(P.seed, gid, count, 3), r4 = hand_rand(P.seed, gid, count, 4);
+    if (P.object_is_pen) t_randomize_rotation_pen(r3, ob.q);
+    else t_randomize_rotation(r3, r4, ob.q);
+#pragma unroll
+    for (int c = 0; c < 3; c++) { ob.v[c] = 0.f; ob.w[c] = 0.f; }
+}
+__device__ __forceinline__ float2 hand_reset_dof(const b2g_hand_params &P, uint32_t gid, uint32_t count, int d, int nd) {
+    const float delta_max = P.dof_upper[d] - P.dof_default_pos[d], delta_min = P.dof_lower[d] - P.dof_default_pos[d];
+    const float rand_delta = delta_min + (delta_max - delta_min) * 0.5f * (hand_rand(P.seed, gid, count, 5 + d) + 1.0f);
+    return make_float2(P.dof_default_pos[d] + P.reset_dof_pos_noise * rand_delta,
+                       P.dof_default_vel[d] + P.reset_dof_vel_noise * hand_rand(P.seed, gid, count, 5 + nd + d));
 }
 
 // ---- random forces on the object (shadow_hand.py:700-709, forceScale > 0).  The reference draws from torch's global generator;
@@ -122,28 +159,10 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
     const uint32_t gid = (uint32_t)(e + P.env_id_offset);
     const uint32_t count = do_reset ? (uint32_t)rc[e] : 0u;
 
-    // ---- pre_physics_step: reset_target_pose (:594-610).  An env that resets draws its goal inside reset_idx (:620),
-    // which overrides the goal-only draw of :667-670; a goal-only reset uses its own counter-keyed stream.
+    // ---- pre_physics_step: reset_target_pose.  An env that resets draws its goal inside reset_idx, which overrides :667-670
     float goal_pos[3], goal_rot[4];
     if (do_goal) {
-        float r0, r1;
-        if (do_reset) { r0 = hand_rand(P.seed, gid, count, 2 * nd + 5); r1 = hand_rand(P.seed, gid, count, 2 * nd + 6); }
-        else {
-            const uint32_t gc = (uint32_t)grc[e] | 0x80000000u;
-            r0 = hand_rand(P.seed, gid, gc, 0); r1 = hand_rand(P.seed, gid, gc, 1);
-            if (w0) grc[e] = (int)(((uint32_t)grc[e] + 1u) & 0x7fffffffu);
-        }
-        t_randomize_rotation(r0, r1, goal_rot);
-#pragma unroll
-        for (int c = 0; c < 3; c++) goal_pos[c] = init_rows[26 + c];
-        if (w0) {
-#pragma unroll
-            for (int c = 0; c < 3; c++) { goal_row[c] = goal_pos[c]; rows[26 + c] = goal_pos[c] + P.goal_displacement[c]; }
-#pragma unroll
-            for (int c = 0; c < 4; c++) { goal_row[3 + c] = goal_rot[c]; rows[29 + c] = goal_rot[c]; }
-#pragma unroll
-            for (int c = 7; c < 13; c++) rows[26 + c] = 0.f;
-        }
+        hand_reset_goal(P, gid, count, nd, !do_reset, grc + e, init_rows, goal_row, rows, w0, goal_pos, goal_rot);
     } else {
 #pragma unroll
         for (int c = 0; c < 3; c++) goal_pos[c] = goal_row[c];
@@ -152,13 +171,7 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
     }
     // ---- reset_idx (:612-659): object pose, then the hand's joints and targets
     if (do_reset) {
-        const float rx = hand_rand(P.seed, gid, count, 0), ry = hand_rand(P.seed, gid, count, 1), rz = hand_rand(P.seed, gid, count, 2);
-        ob.p[0] = init_rows[13] + P.reset_position_noise * rx;
-        ob.p[1] = init_rows[14] + P.reset_position_noise * ry;
-        ob.p[2] = init_rows[15] + P.reset_position_noise * rz;
-        t_object_reset_rotation(P, hand_rand(P.seed, gid, count, 3), hand_rand(P.seed, gid, count, 4), ob.q);
-#pragma unroll
-        for (int c = 0; c < 3; c++) { ob.v[c] = 0.f; ob.w[c] = 0.f; }
+        hand_reset_obj(P, gid, count, init_rows, ob);
         progress = 0; successes = 0.f;
         if (w0) rc[e] = (int)(count + 1u);
     }
@@ -171,12 +184,8 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
         float cur = cur_t[d], prev = prev_t[d];
         const float lo = P.dof_lower[d], hi = P.dof_upper[d];
         if (do_reset) {
-            const float delta_max = hi - P.dof_default_pos[d], delta_min = lo - P.dof_default_pos[d];
-            const float rand_delta = delta_min + (delta_max - delta_min) * 0.5f * (hand_rand(P.seed, gid, count, 5 + d) + 1.0f);
-            const float pos = P.dof_default_pos[d] + P.reset_dof_pos_noise * rand_delta;
-            qv.x = pos;
-            qv.y = P.dof_default_vel[d] + P.reset_dof_vel_noise * hand_rand(P.seed, gid, count, 5 + nd + d);
-            cur = pos; prev = pos;
+            qv = hand_reset_dof(P, gid, count, d, nd);
+            cur = qv.x; prev = qv.x;
         }
         const int k = H.dof_action[d];
         if (k >= 0) {
@@ -212,9 +221,8 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
     typename ST::Outputs o;
     o.write = valid;
     o.net_contact = B.p[B2G_T_NET_CONTACT] ? (float *)B.p[B2G_T_NET_CONTACT] + (size_t)e * sm.nb * 3 : nullptr;
-    float *const g_sens = B.p[B2G_T_FORCE_SENSOR] ? (float *)B.p[B2G_T_FORCE_SENSOR] + (size_t)e * sm.nsens * 6 : nullptr;
-    float *const g_dfrc = B.p[B2G_T_DOF_FORCE] ? (float *)B.p[B2G_T_DOF_FORCE] + (size_t)e * nd : nullptr;
-    o.sensor = g_sens; o.dof_force = g_dfrc;
+    o.sensor = B.p[B2G_T_FORCE_SENSOR] ? (float *)B.p[B2G_T_FORCE_SENSOR] + (size_t)e * sm.nsens * 6 : nullptr;
+    o.dof_force = B.p[B2G_T_DOF_FORCE] ? (float *)B.p[B2G_T_DOF_FORCE] + (size_t)e * nd : nullptr;
     const int total = P.control_freq_inv * sm.substeps;
     for (int k = 0; k < total; k++) st.substep(rs, k == total - 1, o, &ob);
     st.pass1(rs);                                   // link poses of the new state (fingertips)
@@ -247,7 +255,7 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
         if (valid) row_dof[d] = qv;
         put(&LY::o_dofpos, d, t_unscale(qv.x, P.dof_lower[d], P.dof_upper[d]));
         put(&LY::o_dofvel, d, P.vel_obs_scale * qv.y);
-        put(&LY::o_dofforce, d, P.force_torque_obs_scale * (g_dfrc ? g_dfrc[d] : 0.f));
+        put(&LY::o_dofforce, d, P.force_torque_obs_scale * (o.dof_force ? o.dof_force[d] : 0.f));
         const int k = H.dof_action[d];
         if (k >= 0) {
             const float a = fminf(fmaxf(actions_in[(size_t)e * NA + k], -P.clip_actions), P.clip_actions);
@@ -285,7 +293,7 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
         put_ft(obs, obsc, H.lay[0]);
         put_ft(states, nullptr, H.lay[1]);
 #pragma unroll
-        for (int c = 0; c < 6; c++) put(&LY::o_sens, 6 * f + c, P.force_torque_obs_scale * (g_sens ? g_sens[6 * f + c] : 0.f));
+        for (int c = 0; c < 6; c++) put(&LY::o_sens, 6 * f + c, P.force_torque_obs_scale * (o.sensor ? o.sensor[6 * f + c] : 0.f));
     }
     action_penalty = lane_sum<L>(action_penalty);
 

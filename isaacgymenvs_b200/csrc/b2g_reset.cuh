@@ -1,7 +1,7 @@
 // b2g_reset.cuh -- VecTask.reset_done() (tasks/base/vec_task.py:440-455): `reset_idx(nonzero(reset_buf))` right at
 // the call, for callers that reset outside step() (rl_games' env wrapper calls it once before the first rollout).
-// The fused step kernels perform the same reset_idx for flagged envs inside the step; these small kernels run the
-// identical arithmetic (same Philox stream: seed, global env id, reset count) on their own, one thread per env,
+// The fused step kernels perform the same reset_idx for flagged envs inside the step; these small kernels call the
+// step kernels' reset helpers (same Philox stream: seed, global env id, reset count) on their own, one thread per env,
 // and clear reset_buf, so the next step finds nothing to reset -- exactly the reference's order of events.
 // Observations are NOT recomputed (the reference's reset_idx does not either: obs_buf is refreshed by the next step).
 #pragma once
@@ -21,14 +21,12 @@ __global__ void __launch_bounds__(128) loco_reset_kernel(Buffers B, const __grid
     const uint32_t count = (uint32_t)rc[e], gid = (uint32_t)(e + P.env_id_offset);
     float2 *const dof = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
     if (P.task == B2G_TASK_CARTPOLE) {
-        for (int s = 0; s < 2; s++)
-            dof[s] = make_float2(0.2f * (reset_uniform(P.seed, gid, count, s) - 0.5f), 0.5f * (reset_uniform(P.seed, gid, count, 2 + s) - 0.5f));
+        for (int s = 0; s < 2; s++) dof[s] = cartpole_reset_dof(P, gid, count, s);
     } else {
         for (int d = 0; d < nd; d++) dof[d] = loco_reset_dof(P, gid, count, d, nd);
-        const float *ir = (const float *)B.p[B2G_T_INITIAL_ROOT] + 13 * (size_t)e;
-        float *r = (float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e;
-        for (int c = 0; c < 13; c++) r[c] = ir[c];
-        const float pot = loco_potential(P, ir);
+        RootState rs;
+        const float pot = loco_reset_root(P, B, e, rs);
+        store_root((float *)B.p[B2G_T_ROOT_STATE] + 13 * (size_t)e, rs);
         ((float *)B.p[B2G_T_POTENTIALS])[e] = pot;                       // prev_potentials = potentials = -|to_target| / dt (:273-276)
         ((float *)B.p[B2G_T_PREV_POTENTIALS])[e] = pot;
     }
@@ -49,27 +47,16 @@ __global__ void __launch_bounds__(128) hand_reset_kernel(Buffers B, const __grid
     float *const rows = (float *)B.p[B2G_T_ROOT_STATE] + (size_t)e * 39;
     const float *const init_rows = (const float *)B.p[B2G_T_INITIAL_ROOT] + (size_t)e * 39;
     float *const goal_row = (float *)B.p[B2G_T_GOAL_STATES] + (size_t)e * 13;
-    float goal_rot[4];
-    t_randomize_rotation(hand_rand(P.seed, gid, count, 2 * nd + 5), hand_rand(P.seed, gid, count, 2 * nd + 6), goal_rot);
-    for (int c = 0; c < 3; c++) { goal_row[c] = init_rows[26 + c]; rows[26 + c] = init_rows[26 + c] + P.goal_displacement[c]; }
-    for (int c = 0; c < 4; c++) { goal_row[3 + c] = goal_rot[c]; rows[29 + c] = goal_rot[c]; }
-    for (int c = 7; c < 13; c++) rows[26 + c] = 0.f;
-    float oq[4];
-    rows[13] = init_rows[13] + P.reset_position_noise * hand_rand(P.seed, gid, count, 0);
-    rows[14] = init_rows[14] + P.reset_position_noise * hand_rand(P.seed, gid, count, 1);
-    rows[15] = init_rows[15] + P.reset_position_noise * hand_rand(P.seed, gid, count, 2);
-    t_object_reset_rotation(P, hand_rand(P.seed, gid, count, 3), hand_rand(P.seed, gid, count, 4), oq);
-    for (int c = 0; c < 4; c++) rows[16 + c] = oq[c];
-    for (int c = 7; c < 13; c++) rows[13 + c] = 0.f;
+    float goal_pos[3], goal_rot[4];
+    hand_reset_goal(P, gid, count, nd, false, nullptr, init_rows, goal_row, rows, true, goal_pos, goal_rot);
+    ObjState ob;
+    hand_reset_obj(P, gid, count, init_rows, ob);
+    store_obj(rows + 13, ob);
     float2 *const dof = (float2 *)B.p[B2G_T_DOF_STATE] + (size_t)e * nd;
     float *const cur_t = (float *)B.p[B2G_T_DOF_TARGET] + (size_t)e * nd, *const prev_t = (float *)B.p[B2G_T_PREV_TARGETS] + (size_t)e * nd;
     for (int d = 0; d < nd; d++) {
-        const float lo = P.dof_lower[d], hi = P.dof_upper[d];
-        const float delta_max = hi - P.dof_default_pos[d], delta_min = lo - P.dof_default_pos[d];
-        const float rand_delta = delta_min + (delta_max - delta_min) * 0.5f * (hand_rand(P.seed, gid, count, 5 + d) + 1.0f);
-        const float pos = P.dof_default_pos[d] + P.reset_dof_pos_noise * rand_delta;
-        dof[d] = make_float2(pos, P.dof_default_vel[d] + P.reset_dof_vel_noise * hand_rand(P.seed, gid, count, 5 + nd + d));
-        cur_t[d] = pos; prev_t[d] = pos;
+        const float2 qv = hand_reset_dof(P, gid, count, d, nd);
+        dof[d] = qv; cur_t[d] = qv.x; prev_t[d] = qv.x;
     }
     if (P.force_scale > 0.f) {                                           // rb_forces[env_ids] = 0, new random_force_prob (:616,642)
         float *const of = (float *)B.p[B2G_T_OBJ_FORCE] + 3 * (size_t)e;

@@ -237,6 +237,10 @@ __device__ __forceinline__ void cartpole_reward(float pole_angle, float pole_vel
     if ((float)progress >= max_len - 1.f) reset = 1;
     rew = reward;
 }
+// reset_idx, cartpole.py:144-157: DOF s (0 cart, 1 pole) of env `gid`'s reset number `count` -- (position, velocity)
+__device__ __forceinline__ float2 cartpole_reset_dof(const b2g_task_params &P, uint32_t gid, uint32_t count, int s) {
+    return make_float2(0.2f * (reset_uniform(P.seed, gid, count, s) - 0.5f), 0.5f * (reset_uniform(P.seed, gid, count, 2 + s) - 0.5f));
+}
 
 // ------------------------------------------------------------------ AnymalTerrain helpers (tasks/anymal_terrain.py)
 // uniform in [0,1) number `idx` of stream (env, step, tag)
