@@ -29,52 +29,6 @@ __device__ __forceinline__ void load_model_full(DevModel *sm, const DevModel *__
     __syncthreads();
 }
 
-// Step-kernel prologue: ONE mbarrier transaction brings the hot part of the model (header, links,
-// contact spheres) and, when the block owns whole 16-byte-aligned tiles, this block's slice of
-// root_state / dof_state / actions into shared memory with bulk-async (TMA) copies.
-struct Tiles {
-    const float *root;     // [envs_per_block][13]   (shared memory, or global when !on)
-    const float2 *dof;     // [envs_per_block][nd]
-    const float *act;      // [envs_per_block][na]
-    bool on;
-};
-__device__ __forceinline__ uint32_t round16(uint32_t b) { return (b + 15u) & ~15u; }
-
-__device__ __forceinline__ Tiles prologue(DevModel *sm, uint64_t *mbar, const DevModel *__restrict__ gm, float4 *tile_smem,
-                                          bool tiles_on, int env0, int epb, const float *g_root, const float *g_dof,
-                                          const float *g_act, int nd_hint, int na_hint) {
-    Tiles t;
-    if (threadIdx.x == 0) mbar_init(mbar, 1);
-    __syncthreads();
-    const uint32_t rb = (uint32_t)epb * 13u * 4u, db = (uint32_t)epb * (uint32_t)nd_hint * 8u, ab = (uint32_t)epb * (uint32_t)na_hint * 4u;
-    float *s_root = reinterpret_cast<float *>(tile_smem);
-    float *s_dof = s_root + rb / 4;
-    float *s_act = s_dof + db / 4;
-    if (threadIdx.x == 0) {
-        const int nl = gm->nl, ncp = gm->ncp, ns = gm->ns;   // three scalar loads; everything else arrives by bulk copy
-        const uint32_t hb = (uint32_t)offsetof(DevModel, slots) + (uint32_t)ns * MAX_LANES * (uint32_t)sizeof(SlotRec);
-        const uint32_t lb = round16((uint32_t)nl * (uint32_t)sizeof(LinkC)), cb = round16((uint32_t)ncp * (uint32_t)sizeof(CpC));
-        uint32_t total = hb + lb + cb;
-        if (tiles_on) total += rb + db + (g_act ? ab : 0u);
-        mbar_expect_tx(mbar, total);
-        bulk_g2s(sm, gm, hb, mbar);
-        bulk_g2s(sm->links, gm->links, lb, mbar);
-        if (cb) bulk_g2s(sm->cps, gm->cps, cb, mbar);
-        if (tiles_on) {
-            bulk_g2s(s_root, g_root + (size_t)env0 * 13, rb, mbar);
-            bulk_g2s(s_dof, g_dof + (size_t)env0 * nd_hint * 2, db, mbar);
-            if (g_act) bulk_g2s(s_act, g_act + (size_t)env0 * na_hint, ab, mbar);
-        }
-    }
-    mbar_wait(mbar, 0);
-    t.on = tiles_on;
-    t.root = tiles_on ? s_root : g_root + (size_t)env0 * 13;
-    t.dof = reinterpret_cast<const float2 *>(tiles_on ? s_dof : g_dof + (size_t)env0 * nd_hint * 2);
-    t.act = g_act ? (tiles_on ? s_act : g_act + (size_t)env0 * na_hint) : nullptr;
-    return t;
-}
-
-
 template <int L, bool HF, int BLOCK, bool OBJ = false, bool SELF = false, bool DR = false>
 __device__ __forceinline__ Stepper<L, HF, BLOCK, OBJ, SELF, DR> make_stepper(const DevModel *sm, const int16_t *hf, int lane) {
     Stepper<L, HF, BLOCK, OBJ, SELF, DR> st;
@@ -144,7 +98,7 @@ __global__ void __launch_bounds__(BLOCK) simulate_kernel(const DevModel *__restr
                                                          Buffers B, int N) {
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
-    prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
+    load_model_hot(&sm, &mbar, gm);
     using ST = Stepper<L, HF, BLOCK, OBJ, SELF, DR>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;
@@ -188,11 +142,9 @@ __global__ void __launch_bounds__(BLOCK) simulate_kernel(const DevModel *__restr
 // -------------------------------------------------------------------------------------------
 // One whole VecTask.step() of Ant / Humanoid (vec_task.py:360-408 + ant.py:281-297 / humanoid.py)
 //
-// Data movement: with whole 16-byte-aligned tiles per block (tiles_on) every tensor of the step
-// moves as ONE bulk-async copy per block: in  -- model, root_state, dof_state, actions;
-// out -- root_state, dof_state, clamped actions, force sensors, dof forces, obs (+ clipped obs),
-// rew, reset, progress, potentials, prev_potentials, up_vec, heading_vec, time-outs.  The output
-// tiles are staged in the shared memory that held the slot state during the physics.
+// Data movement: with whole 16-byte-aligned tiles per block (TILES) every tensor of the step moves as ONE bulk-async
+// copy per block (the tile helpers of b2g_common.cuh); the output tiles are staged in the shared memory that held the
+// slot state during the physics.  Without tiles the kernel reads and writes the tensors directly.
 #ifndef B2G_MINBLOCKS
 #define B2G_MINBLOCKS 4
 #endif
@@ -212,17 +164,11 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     const int env0 = blockIdx.x * EPB;
     constexpr bool tiles = TILES;
     float *const io = reinterpret_cast<float *>(b2g_dyn_smem + ta.io_f4);
-    // ---- in/out tile region: root | dof | act | sensors | dof_force
     const int nsens6 = 6 * ((P.num_obs - 12 - (HUM ? 4 : 3) * nd) / 6);          // 6 * nsens, from the obs layout
-    float *const s_root = io;
-    float *const s_dof = s_root + EPB * 13;
-    float *const s_act = s_dof + EPB * nd * 2;
-    float *const s_sens = s_act + EPB * nd;
-    float *const s_dfrc = s_sens + EPB * nsens6;
-    // ---- prologue.  Programmatic dependent launch: this grid may start while the previous kernel in the
-    // stream (the previous control step) is still draining.  Everything that does not depend on it --
-    // barrier set-up and the bulk copy of the (constant) model -- happens before griddepcontrol.wait;
-    // the state tiles and per-env scalars are fetched after it.
+    const TileLayout tl = tile_layout(EPB, nd, nsens6, HUM);
+    float *const s_root = io, *const s_dof = io + tl.dof, *const s_act = io + tl.act, *const s_sens = io + tl.sens, *const s_dfrc = io + tl.dfrc;
+    // ---- prologue: barrier set-up and the bulk copy of the (constant) model before griddepcontrol.wait, the state tiles
+    // and per-env scalars after it
     __shared__ alignas(8) uint64_t mbar2;
     long long *const progress_b = (long long *)B.p[B2G_T_PROGRESS];
     long long *const reset_b = (long long *)B.p[B2G_T_RESET];
@@ -231,29 +177,14 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     if (threadIdx.x == 0) { mbar_init(&mbar, 1); mbar_init(&mbar2, 1); }
     __syncthreads();
     if (threadIdx.x == 0) {
-        const int nl = gm->nl, ncp = gm->ncp, ns = gm->ns;   // three scalar loads; everything else arrives by bulk copy
-        const uint32_t hb = (uint32_t)offsetof(DevModel, slots) + (uint32_t)ns * MAX_LANES * (uint32_t)sizeof(SlotRec);
-        const uint32_t lb = round16((uint32_t)nl * (uint32_t)sizeof(LinkC)), cb = round16((uint32_t)ncp * (uint32_t)sizeof(CpC));
-        mbar_expect_tx(&mbar, hb + lb + cb);
-        bulk_g2s(&sm, gm, hb, &mbar);                                      // header | slots[0..ns)
-        char *const pk = reinterpret_cast<char *>(&sm) + hb;               // links and cps packed right behind
-        bulk_g2s(pk, gm->links, lb, &mbar);
-        if (cb) bulk_g2s(pk + lb, gm->cps, cb, &mbar);
+        const ModelHot h = model_hot_bytes(gm->ns, gm->nl, gm->ncp);   // three scalar loads; everything else arrives by bulk copy
+        mbar_expect_tx(&mbar, h.total());
+        bulk_g2s(&sm, gm, h.head, &mbar);                                  // header | slots[0..ns)
+        char *const pk = reinterpret_cast<char *>(&sm) + h.head;           // links and cps packed right behind
+        bulk_g2s(pk, gm->links, h.links, &mbar);
+        if (h.cps) bulk_g2s(pk + h.links, gm->cps, h.cps, &mbar);
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");                     // previous step's writes are now visible
-    if (tiles && threadIdx.x == 0) {
-        const uint32_t rb = EPB * 13 * 4, db = (uint32_t)(EPB * nd * 8), ab = (uint32_t)(EPB * nd * 4);
-        mbar_expect_tx(&mbar2, rb + db + (HOSTIO ? 0u : ab));
-        bulk_g2s(s_root, (const float *)B.p[B2G_T_ROOT_STATE] + (size_t)env0 * 13, rb, &mbar2);
-        bulk_g2s(s_dof, (const float *)B.p[B2G_T_DOF_STATE] + (size_t)env0 * nd * 2, db, &mbar2);
-        if (!HOSTIO) bulk_g2s(s_act, actions_in + (size_t)env0 * nd, ab, &mbar2);
-    }
-    if (tiles && HOSTIO) {         // actions straight from pinned host memory
-        const float4 *src = reinterpret_cast<const float4 *>(ta.h_act + (size_t)env0 * nd);
-        float4 *dst = reinterpret_cast<float4 *>(s_act);
-        for (int i = threadIdx.x; i < EPB * nd / 4; i += BLOCK) dst[i] = src[i];
-        __syncthreads();
-    }
+    load_state_tiles<EPB, BLOCK, TILES, HOSTIO>(&mbar2, io, tl, B, nd, actions_in, env0, ta);
     // per-env scalars of post_physics_step: issued now, consumed after the physics
     const long long progress_in = progress_b[e_pre];
     const long long reset_in = reset_b[e_pre];
@@ -273,6 +204,7 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     attach_env_params_generic(st, sm, B, e);
     if (DR) st.dr_grav = (const float *)B.p[B2G_T_GRAVITY];
     {
+        // model_hot_bytes's layout with 64-bit offset arithmetic: its 32-bit form costs the Humanoid DR instantiations registers
         const char *pk = reinterpret_cast<const char *>(&sm) + offsetof(DevModel, slots) + (size_t)sm.ns * MAX_LANES * sizeof(SlotRec);
         st.links = reinterpret_cast<const LinkC *>(pk);
         st.gr.cps = reinterpret_cast<const CpC *>(pk + round16((uint32_t)sm.nl * (uint32_t)sizeof(LinkC)));
@@ -397,10 +329,7 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
         float *uv = (float *)B.p[B2G_T_UP_VEC], *hv = (float *)B.p[B2G_T_HEADING_VEC];
         uint8_t *to = (uint8_t *)B.p[B2G_T_TIMEOUT];
         if (tiles) {
-            t.rew[el] = total_r; t.reset[el] = reset; t.prog[el] = progress; t.pot[el] = potentials; t.ppot[el] = prev_potentials;
-            t.up[3 * el] = ro.up_vec[0]; t.up[3 * el + 1] = ro.up_vec[1]; t.up[3 * el + 2] = ro.up_vec[2];
-            t.head[3 * el] = ro.heading_vec[0]; t.head[3 * el + 1] = ro.heading_vec[1]; t.head[3 * el + 2] = ro.heading_vec[2];
-            t.to[el] = tout;
+            stage_row(t, el, total_r, r.died || r.timed, progress, potentials, prev_potentials, ro.up_vec, ro.heading_vec, r.timed);
         } else {
             ((float *)B.p[B2G_T_REW])[e] = total_r;
             reset_b[e] = reset; progress_b[e] = progress;
@@ -413,26 +342,8 @@ __global__ void __launch_bounds__(BLOCK, (BLOCK == 128 ? B2G_MINBLOCKS : (BLOCK 
     if (tiles) {
         fence_async_smem();
         __syncthreads();
-        if (threadIdx.x == 0) {
-            const size_t e0 = (size_t)env0;
-            if (!sm.root_fixed) bulk_s2g((float *)B.p[B2G_T_ROOT_STATE] + e0 * 13, s_root, EPB * 13 * 4);
-            bulk_s2g((float *)B.p[B2G_T_DOF_STATE] + e0 * nd * 2, s_dof, (uint32_t)(EPB * nd * 8));
-            if (g_act_out) bulk_s2g(g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
-            if (stage_out && g_sens && nsens6) bulk_s2g(g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
-            if (stage_out && HUM && g_dfrc) bulk_s2g(g_dfrc + e0 * nd, s_dfrc, (uint32_t)(EPB * nd * 4));
-            bulk_s2g(g_obs + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
-            if (g_obsc) bulk_s2g(g_obsc + e0 * O, t.obsc, (uint32_t)(EPB * O * 4));
-            bulk_s2g((float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
-            bulk_s2g(pot_b + e0, t.pot, EPB * 4);
-            bulk_s2g(ppot_b + e0, t.ppot, EPB * 4);
-            if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, t.up, EPB * 12);
-            if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t.head, EPB * 12);
-            bulk_s2g(reset_b + e0, t.reset, EPB * 8);
-            bulk_s2g(progress_b + e0, t.prog, EPB * 8);
-            if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
-
-            bulk_commit_wait();
-        }
+        // one issuing thread, as before: dealt across the warps, the Humanoid step measured no faster (H100, 700 W)
+        drain_tiles<EPB, 1, HUM>(B, t, io, tl, s_act, nd, O, nsens6, env0, !sm.root_fixed, stage_out, true);
         if (HOSTIO) loco_copy_to_host<BLOCK>(ta, t, (size_t)env0, EPB, O, g_obsc != nullptr);
     }
 }
@@ -445,7 +356,7 @@ __global__ void __launch_bounds__(BLOCK) cartpole_step_kernel(const DevModel *__
                                                               const float *__restrict__ actions_in, int N) {
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
-    prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
+    load_model_hot(&sm, &mbar, gm);
     using ST = Stepper<1, false, BLOCK>;
     const int env = blockIdx.x * BLOCK + threadIdx.x;
     const bool valid = env < N;
@@ -1064,9 +975,9 @@ struct HostOut {
     uint8_t *timeout;
 };
 
-static TileArgs tile_args(bool on, size_t io_bytes_at, size_t model_bytes_at, const float *actions, const HostOut *io) {
+static TileArgs tile_args(size_t io_bytes_at, size_t model_bytes_at, const float *actions, const HostOut *io) {
     TileArgs ta;
-    ta.on = on ? 1 : 0; ta.io_f4 = (int)(io_bytes_at / 16); ta.model_f4 = (int)(model_bytes_at / 16);
+    ta.io_f4 = (int)(io_bytes_at / 16); ta.model_f4 = (int)(model_bytes_at / 16);
     ta.h_act = io ? actions : nullptr;
     ta.h_obs = io ? io->obs : nullptr; ta.h_rew = io ? io->rew : nullptr; ta.h_reset = io ? io->reset : nullptr; ta.h_timeout = io ? io->timeout : nullptr;
     return ta;
@@ -1108,24 +1019,23 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
     if (!hum && s->quad_ns == 2 && !s->d_hf) {           // Ant on the quad sub-step (whole tiles only)
         constexpr int EPB = QUAD_LOCO_BLOCK / 4, ND = 8;
         const size_t park_bytes = (size_t)quad_park_f4(2) * QUAD_LOCO_BLOCK * sizeof(float4);
-        const size_t io_bytes = ((size_t)EPB * (13 + 3 * ND + ns6) * 4 + 15) & ~(size_t)15;
+        const size_t io_bytes = tile_layout(EPB, ND, ns6, false).bytes;
         if (whole_tiles(N, EPB) && loco_stage_bytes(EPB, O, clip_sep) <= park_bytes) {
             const size_t dyn = park_bytes + io_bytes + (size_t)quad_model_f4(2) * sizeof(float4);
             const bool lean = !s->buf.p[B2G_T_ENV_MASS_SCALE] && !s->buf.p[B2G_T_ENV_DOF_PROPS] && !s->buf.p[B2G_T_ENV_FRICTION] &&
                               !s->buf.p[B2G_T_NET_CONTACT] && !s->buf.p[B2G_T_DOF_FORCE];
             return launch(s, quad_loco_kernel_for(s->quad_spec, io != nullptr, lean), (int)N / EPB, QUAD_LOCO_BLOCK, dyn, st, SMEM_PDL,
                           (const float4 *)s->d_qm, s->buf, P, actions, (int)N, (int)s->hm.substeps,
-                          tile_args(true, park_bytes, park_bytes + io_bytes, actions, io));
+                          tile_args(park_bytes, park_bytes + io_bytes, actions, io));
         }
     }
     if (s->d_hf) return fail(B2G_E_UNSUPPORTED, "locomotion tasks run on the ground plane");
     // tiles by bulk copy: whole blocks only, every tile a multiple of 16 bytes at a 16-byte-aligned address
     const int epb = blk / s->lanes, ndof = s->hm.nl - 1;
     const size_t state_bytes = s->dyn_smem;                                   // slot state + accumulators
-    const size_t io_bytes = ((size_t)epb * (13 + 3 * ndof + ns6 + (hum ? ndof : 0)) * 4 + 15) & ~(size_t)15;
+    const size_t io_bytes = tile_layout(epb, ndof, ns6, hum).bytes;
     const bool tiles = whole_tiles(N, epb) && loco_stage_bytes(epb, O, clip_sep) <= state_bytes && s->buf.p[B2G_T_ACTIONS];
-    const size_t model_bytes = offsetof(DevModel, slots) + (size_t)s->hm.ns * MAX_LANES * sizeof(SlotRec) + (((size_t)s->hm.nl * sizeof(LinkC) + 15) & ~(size_t)15) +
-                               (((size_t)s->hm.ncp * sizeof(CpC) + 15) & ~(size_t)15);
+    const size_t model_bytes = model_hot_bytes(s->hm.ns, s->hm.nl, s->hm.ncp).total();
     const size_t io_used = tiles ? io_bytes : 16;
     const size_t dyn = state_bytes + io_used + model_bytes;
     const LocoKernel k = loco_kernel_for(s->lanes, blk, hum, tiles, io != nullptr, s->hm.self_on, grav);
@@ -1136,7 +1046,7 @@ static int task_step(b2g_sim *s, const float *actions, void *stream, const HostO
         return fail(B2G_E_UNSUPPORTED, std::string("no locomotion step kernel instantiated for this combination ") + what);
     }
     return launch(s, k, grid, blk, dyn, st, SMEM_PDL, (const DevModel *)s->dm, (const int16_t *)s->d_hf, s->buf, P, actions, (int)N,
-                  tile_args(tiles, state_bytes, state_bytes + io_used, actions, io));
+                  tile_args(state_bytes, state_bytes + io_used, actions, io));
 }
 
 // the fused Ant step on the quad sub-step: (specialisation, host I/O, lean); 64 threads, 16 envs per CTA.  Lean: the plain
@@ -1225,7 +1135,7 @@ extern "C" int b2g_task_rollout(b2g_sim *s, const float *actions, int32_t K, flo
     CUDA_TRY(cudaSetDevice(s->device));
     const int nd_ = 8, O = P.num_obs, ns6 = 6 * s->hm.nsens;
     const size_t park_f4 = (size_t)quad_park_f4(2) * QB;
-    const size_t io_f4 = ((size_t)EPB * (13 + 2 * nd_ + 2 * nd_ + ns6) * 4 + 15) / 16;
+    const size_t io_f4 = tile_layout(EPB, nd_, ns6, false, 2).bytes / 16;
     const size_t model_f4 = quad_model_f4(2);
     const size_t stage_f4 = (roll_stage_bytes(EPB, O) + 15) / 16;
     if (roll_last_bytes(EPB, O) > park_f4 * 16) return fail(B2G_E_UNSUPPORTED, "b2g_task_rollout: observation too large for the last-step staging");

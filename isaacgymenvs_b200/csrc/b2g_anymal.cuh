@@ -24,7 +24,7 @@ __global__ void __launch_bounds__(128) anymal_physics_kernel(const DevModel *__r
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
     __shared__ float s_part[BLOCK / 32];
-    prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
+    load_model_hot(&sm, &mbar, gm);
     using ST = Stepper<L, HF, BLOCK>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;

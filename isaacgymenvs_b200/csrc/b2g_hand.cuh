@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(BLOCK) hand_step_kernel(const DevModel *__rest
                                                           const float *__restrict__ actions_in, int N) {
     __shared__ DevModel sm;
     __shared__ alignas(8) uint64_t mbar;
-    prologue(&sm, &mbar, gm, nullptr, false, 0, 0, nullptr, nullptr, nullptr, 0, 0);
+    load_model_hot(&sm, &mbar, gm);
     using ST = Stepper<L, false, BLOCK, true, false, DR>;
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int env = gt / L, lane = gt % L;

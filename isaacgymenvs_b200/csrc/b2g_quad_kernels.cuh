@@ -176,38 +176,22 @@ __global__ void __launch_bounds__(BLOCK, B2G_QUAD_MINBLOCKS(BLOCK)) quad_loco_ke
     const int O = P.num_obs;
     const int nsens6 = O - 12 - 3 * nd;                      // 6 * nsens, from the obs layout (checked by b2g_set_task)
     const int env0 = blockIdx.x * EPB;
-    // ---- in/out tile region: root | dof | act | sensors
-    float *const s_root = io;
-    float *const s_dof = s_root + EPB * 13;
-    float *const s_act = s_dof + EPB * nd * 2;
-    float *const s_sens = s_act + EPB * nd;
+    const TileLayout tl = tile_layout(EPB, nd, nsens6, false);
+    float *const s_root = io, *const s_dof = io + tl.dof, *const s_act = io + tl.act, *const s_sens = io + tl.sens;
     long long *const progress_b = (long long *)B.p[B2G_T_PROGRESS];
     long long *const reset_b = (long long *)B.p[B2G_T_RESET];
-    float *const pot_b = (float *)B.p[B2G_T_POTENTIALS], *const ppot_b = (float *)B.p[B2G_T_PREV_POTENTIALS];
+    float *const pot_b = (float *)B.p[B2G_T_POTENTIALS];
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int e = gt >> 2, lane = gt & 3;                    // whole tiles: every env of the block exists
     const int el = e - env0;
-    // ---- prologue (programmatic dependent launch: everything before griddepcontrol.wait overlaps the previous step's tail)
+    // ---- prologue: the model before griddepcontrol.wait, the state tiles after it
     if (threadIdx.x == 0) { mbar_init(&mbar, 1); mbar_init(&mbar2, 1); }
     __syncthreads();
     if (threadIdx.x == 0) {
         mbar_expect_tx(&mbar, quad_model_f4(NS) * 16);
         bulk_g2s(qm, gqm, quad_model_f4(NS) * 16, &mbar);
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (threadIdx.x == 0) {
-        constexpr uint32_t rb = EPB * 13 * 4, db = EPB * nd * 8, ab = EPB * nd * 4;
-        mbar_expect_tx(&mbar2, rb + db + (HOSTIO ? 0u : ab));
-        bulk_g2s(s_root, (const float *)B.p[B2G_T_ROOT_STATE] + (size_t)env0 * 13, rb, &mbar2);
-        bulk_g2s(s_dof, (const float *)B.p[B2G_T_DOF_STATE] + (size_t)env0 * nd * 2, db, &mbar2);
-        if (!HOSTIO) bulk_g2s(s_act, actions_in + (size_t)env0 * nd, ab, &mbar2);
-    }
-    if (HOSTIO) {                  // actions straight from pinned host memory
-        const float4 *src = reinterpret_cast<const float4 *>(ta.h_act + (size_t)env0 * nd);
-        float4 *dst = reinterpret_cast<float4 *>(s_act);
-        for (int i = threadIdx.x; i < EPB * nd / 4; i += BLOCK) dst[i] = src[i];
-        __syncthreads();
-    }
+    load_state_tiles<EPB, BLOCK, true, HOSTIO>(&mbar2, io, tl, B, nd, actions_in, env0, ta);
     const long long progress_in = progress_b[e];
     const long long reset_in = reset_b[e];
     const float potentials_in = pot_b[e];
@@ -293,47 +277,13 @@ __global__ void __launch_bounds__(BLOCK, B2G_QUAD_MINBLOCKS(BLOCK)) quad_loco_ke
     cost.sum_lanes<4>();
     if (lane == 0) {
         const LocoReward r = loco_reward(P, ro.up_proj, ro.heading_proj, potentials, prev_potentials, cost, rs.rp[2], progress, false);
-        t.rew[el] = r.rew; t.reset[el] = (r.died || r.timed) ? 1 : 0; t.prog[el] = progress; t.pot[el] = potentials; t.ppot[el] = prev_potentials;
-        t.up[3 * el] = ro.up_vec[0]; t.up[3 * el + 1] = ro.up_vec[1]; t.up[3 * el + 2] = ro.up_vec[2];
-        t.head[3 * el] = ro.heading_vec[0]; t.head[3 * el + 1] = ro.heading_vec[1]; t.head[3 * el + 2] = ro.heading_vec[2];
-        t.to[el] = r.timed;
+        stage_row(t, el, r.rew, r.died || r.timed, progress, potentials, prev_potentials, ro.up_vec, ro.heading_vec, r.timed);
     }
     fence_async_smem();
     __syncthreads();
-    // one bulk-async (TMA) store per output tensor.  The stores are dealt to the FIRST THREAD of each warp at compile time
-    // (`threadIdx.x == 32 w` branches, each a single-thread region the compiler keeps on the uniform datapath): their issue
-    // -- address arithmetic + UBLKCP each -- runs in parallel instead of as one thread's serial tail
     static_assert(EPB % 16 == 0, "bulk copies move multiples of 16 bytes: the timeout tile is EPB bytes");
-    const size_t e0 = (size_t)env0;
-    {
-        float *const g_act_out = (float *)B.p[B2G_T_ACTIONS];
-        constexpr int NW = BLOCK / 32;
-        auto issue = [&](int w) {
-            int k = 0;
-#define B2G_ST(COND, DST, SRC, BYTES) do { if ((k++ % NW) == w) { if (COND) bulk_s2g(DST, SRC, BYTES); } } while (0)
-            B2G_ST(true, g_obs + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
-            B2G_ST(g_obsc != nullptr, g_obsc + e0 * O, t.obsc, (uint32_t)(EPB * O * 4));
-            B2G_ST(true, (float *)B.p[B2G_T_ROOT_STATE] + e0 * 13, s_root, EPB * 13 * 4);
-            B2G_ST(true, (float *)B.p[B2G_T_DOF_STATE] + e0 * nd * 2, s_dof, (uint32_t)(EPB * nd * 8));
-            B2G_ST(g_act_out != nullptr, g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
-            B2G_ST(stage_out && g_sens && nsens6, g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
-            B2G_ST(true, (float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
-            B2G_ST(true, pot_b + e0, t.pot, EPB * 4);
-            B2G_ST(true, ppot_b + e0, t.ppot, EPB * 4);
-            B2G_ST(B.p[B2G_T_UP_VEC] != nullptr, (float *)B.p[B2G_T_UP_VEC] + 3 * e0, t.up, EPB * 12);
-            B2G_ST(B.p[B2G_T_HEADING_VEC] != nullptr, (float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, t.head, EPB * 12);
-            B2G_ST(true, reset_b + e0, t.reset, EPB * 8);
-            B2G_ST(true, progress_b + e0, t.prog, EPB * 8);
-            B2G_ST(B.p[B2G_T_TIMEOUT] != nullptr, (uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
-#undef B2G_ST
-            bulk_commit_wait();
-        };
-        if (threadIdx.x == 0) issue(0);
-        else if (NW > 1 && threadIdx.x == 32) issue(1);
-        else if (NW > 2 && threadIdx.x == 64) issue(2);
-        else if (NW > 3 && threadIdx.x == 96) issue(3);
-    }
-    if (HOSTIO) loco_copy_to_host<BLOCK>(ta, t, e0, EPB, O, g_obsc != nullptr);
+    drain_tiles<EPB, BLOCK / 32, false>(B, t, io, tl, s_act, nd, O, nsens6, env0, true, stage_out, true);
+    if (HOSTIO) loco_copy_to_host<BLOCK>(ta, t, (size_t)env0, EPB, O, g_obsc != nullptr);
 }
 
 

@@ -33,10 +33,6 @@ struct RollStage {
     long long *reset;
     uint8_t *to;
 };
-struct RollLast {
-    float *obs, *pot, *ppot, *up, *head;
-    long long *prog;
-};
 __device__ __forceinline__ RollStage roll_stage(float *base, int epb, int O) {
     RollStage t;
     t.obs = base;
@@ -45,10 +41,12 @@ __device__ __forceinline__ RollStage roll_stage(float *base, int epb, int O) {
     t.to = reinterpret_cast<uint8_t *>(t.reset + epb);
     return t;
 }
-__device__ __forceinline__ RollLast roll_last(float *base, int epb, int O) {
-    RollLast l;
-    l.obs = base;
-    l.pot = l.obs + epb * O; l.ppot = l.pot + epb; l.up = l.ppot + epb; l.head = l.up + 3 * epb;
+// the last step's results as drain_tiles stores them: the per-step tiles of t, the rest in base (obs: the unclipped copy,
+// written only when a separate clipped tensor exists)
+__device__ __forceinline__ LocoStage roll_last(float *base, const RollStage &t, int epb, int O) {
+    LocoStage l;
+    l.obs = base; l.obsc = t.obs; l.rew = t.rew; l.reset = t.reset; l.to = t.to;
+    l.pot = base + epb * O; l.ppot = l.pot + epb; l.up = l.ppot + epb; l.head = l.up + 3 * epb;
     l.prog = reinterpret_cast<long long *>(l.head + 3 * epb);
     return l;
 }
@@ -67,18 +65,18 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
     const int O = P.num_obs, K = ra.K;
     const int nsens6 = O - 12 - 3 * nd;
     const int env0 = blockIdx.x * EPB;
-    float *const s_root = io;
-    float *const s_dof = s_root + EPB * 13;
-    float *const s_actb[2] = {s_dof + EPB * nd * 2, s_dof + EPB * nd * 2 + EPB * nd};
-    float *const s_sens = s_actb[1] + EPB * nd;
-    const RollStage t = roll_stage(stage, EPB, O);
-    const RollLast l = roll_last(reinterpret_cast<float *>(park), EPB, O);
+    const TileLayout tl = tile_layout(EPB, nd, nsens6, false, 2);
+    float *const s_root = io, *const s_dof = io + tl.dof, *const s_sens = io + tl.sens;
+    float *const s_actb[2] = {io + tl.act, io + tl.act + EPB * nd};
     long long *const progress_b = (long long *)B.p[B2G_T_PROGRESS];
     long long *const reset_b = (long long *)B.p[B2G_T_RESET];
-    float *const pot_b = (float *)B.p[B2G_T_POTENTIALS], *const ppot_b = (float *)B.p[B2G_T_PREV_POTENTIALS];
+    float *const pot_b = (float *)B.p[B2G_T_POTENTIALS];
     float *const g_obs = (float *)B.p[B2G_T_OBS];
     float *g_obsc = (float *)B.p[B2G_T_OBS_CLIPPED];
     if (g_obsc == g_obs) g_obsc = nullptr;
+    const bool clip_sep = g_obsc != nullptr;
+    const RollStage t = roll_stage(stage, EPB, O);
+    const LocoStage l = roll_last(reinterpret_cast<float *>(park), t, EPB, O);
     float *const g_sens = (float *)B.p[B2G_T_FORCE_SENSOR], *const g_dfrc = (float *)B.p[B2G_T_DOF_FORCE];
     const int gt = blockIdx.x * BLOCK + threadIdx.x;
     const int e = gt >> 2, lane = gt & 3;
@@ -90,12 +88,8 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
         mbar_expect_tx(&mbar, quad_model_f4(NS) * 16);
         bulk_g2s(qm, gqm, quad_model_f4(NS) * 16, &mbar);
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    load_state_tiles<EPB, BLOCK, true, false, false>(&mbar2, io, tl, B, nd, nullptr, env0, TileArgs{});
     if (threadIdx.x == 0) {
-        constexpr uint32_t rb = EPB * 13 * 4, db = EPB * nd * 8;
-        mbar_expect_tx(&mbar2, rb + db);
-        bulk_g2s(s_root, (const float *)B.p[B2G_T_ROOT_STATE] + (size_t)env0 * 13, rb, &mbar2);
-        bulk_g2s(s_dof, (const float *)B.p[B2G_T_DOF_STATE] + (size_t)env0 * nd * 2, db, &mbar2);
         mbar_expect_tx(&mbarA[0], ab);
         bulk_g2s(s_actb[0], ra.actions + (size_t)env0 * nd, ab, &mbarA[0]);
     }
@@ -130,7 +124,6 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
     o.sensor = stage_out ? s_sens + nsens6 * el : (g_sens ? g_sens + (size_t)e * nsens6 : nullptr);
     o.dof_force = g_dfrc ? g_dfrc + (size_t)e * nd : nullptr;
     const float clipo = P.clip_obs;
-    const bool clip_sep = g_obsc != nullptr;
     const uint32_t gid = (uint32_t)(e + P.env_id_offset);
 
 #pragma unroll 1
@@ -202,34 +195,20 @@ __global__ void __launch_bounds__(64, 7) quad_rollout_kernel(const float4 *__res
         }
         fence_async_smem();
         __syncthreads();
+        if (last) {
+            LocoStage v = l;                                  // without a separate clipped tensor, obs is the per-step tile
+            if (!clip_sep) v.obs = t.obs;
+            drain_tiles<EPB, BLOCK / 32, false>(B, v, io, tl, s_act, nd, O, nsens6, env0, true, stage_out, false);
+        }
         {
-            const size_t e0 = (size_t)env0, kN = (size_t)kk * N + e0;
+            const size_t kN = (size_t)kk * N + env0;
             if (threadIdx.x == 0) {
                 bulk_s2g(ra.obs_out + kN * O, t.obs, (uint32_t)(EPB * O * 4));
                 bulk_s2g(ra.rew_out + kN, t.rew, EPB * 4);
-                if (last) {
-                    float *const g_act_out = (float *)B.p[B2G_T_ACTIONS];
-                    bulk_s2g(g_obs + e0 * O, clip_sep ? l.obs : t.obs, (uint32_t)(EPB * O * 4));
-                    if (clip_sep) bulk_s2g(g_obsc + e0 * O, t.obs, (uint32_t)(EPB * O * 4));
-                    bulk_s2g((float *)B.p[B2G_T_ROOT_STATE] + e0 * 13, s_root, EPB * 13 * 4);
-                    bulk_s2g((float *)B.p[B2G_T_DOF_STATE] + e0 * nd * 2, s_dof, (uint32_t)(EPB * nd * 8));
-                    if (g_act_out) bulk_s2g(g_act_out + e0 * nd, s_act, (uint32_t)(EPB * nd * 4));
-                }
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             } else if (threadIdx.x == 32) {
                 bulk_s2g(ra.reset_out + kN, t.reset, EPB * 8);
                 if (ra.timeout_out) bulk_s2g(ra.timeout_out + kN, t.to, EPB);
-                if (last) {
-                    if (stage_out && g_sens && nsens6) bulk_s2g(g_sens + e0 * nsens6, s_sens, (uint32_t)(EPB * nsens6 * 4));
-                    bulk_s2g((float *)B.p[B2G_T_REW] + e0, t.rew, EPB * 4);
-                    bulk_s2g(pot_b + e0, l.pot, EPB * 4);
-                    bulk_s2g(ppot_b + e0, l.ppot, EPB * 4);
-                    if (B.p[B2G_T_UP_VEC]) bulk_s2g((float *)B.p[B2G_T_UP_VEC] + 3 * e0, l.up, EPB * 12);
-                    if (B.p[B2G_T_HEADING_VEC]) bulk_s2g((float *)B.p[B2G_T_HEADING_VEC] + 3 * e0, l.head, EPB * 12);
-                    bulk_s2g(reset_b + e0, t.reset, EPB * 8);
-                    bulk_s2g(progress_b + e0, l.prog, EPB * 8);
-                    if (B.p[B2G_T_TIMEOUT]) bulk_s2g((uint8_t *)B.p[B2G_T_TIMEOUT] + e0, t.to, EPB);
-                }
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         }

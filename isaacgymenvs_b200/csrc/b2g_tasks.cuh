@@ -190,41 +190,6 @@ __device__ __forceinline__ LocoReward loco_reward(const b2g_task_params &P, floa
     return r;
 }
 
-// output staging of the fused Ant / Humanoid steps, epb envs per block (floats unless noted):
-// obs | obs_clipped (only when it is a separate tensor) | rew | pot | ppot | up(3) | head(3) | reset(i64) | progress(i64) | timeout(u8)
-struct LocoStage {
-    float *obs, *obsc, *rew, *pot, *ppot, *up, *head;
-    long long *reset, *prog;
-    uint8_t *to;
-};
-__device__ __forceinline__ LocoStage loco_stage(float *base, int epb, int O, bool clip_sep) {
-    LocoStage t;
-    t.obs = base;
-    t.obsc = t.obs + epb * O;
-    t.rew = t.obsc + (clip_sep ? epb * O : 0);
-    t.pot = t.rew + epb; t.ppot = t.pot + epb; t.up = t.ppot + epb; t.head = t.up + 3 * epb;
-    t.reset = reinterpret_cast<long long *>(t.head + 3 * epb); t.prog = t.reset + epb;
-    t.to = reinterpret_cast<uint8_t *>(t.prog + epb);
-    return t;
-}
-__host__ __device__ inline size_t loco_stage_bytes(int epb, int O, bool clip_sep) {
-    return (size_t)epb * ((clip_sep ? 2 : 1) * O * 4 + 4 * 3 + 12 * 2 + 8 * 2 + 1);
-}
-
-// b2g_task_step_host: what VecTask.step returns (vec_task.py:402-408), from the staging tiles straight to the pinned host
-// buffers over PCIe as coalesced 16-byte stores.  Whole tiles only (epb % 16 == 0): every copy is a multiple of 16 bytes.
-template <int BLOCK>
-__device__ __forceinline__ void loco_copy_to_host(const TileArgs &ta, const LocoStage &t, size_t e0, int epb, int O, bool clip_sep) {
-    auto copy16 = [&](void *dst, const void *src, int bytes) {
-        float4 *d = reinterpret_cast<float4 *>(dst); const float4 *sp = reinterpret_cast<const float4 *>(src);
-        for (int i = threadIdx.x; i < bytes / 16; i += BLOCK) d[i] = sp[i];
-    };
-    if (ta.h_obs) copy16(ta.h_obs + e0 * O, clip_sep ? t.obsc : t.obs, epb * O * 4);
-    if (ta.h_rew) copy16(ta.h_rew + e0, t.rew, epb * 4);
-    if (ta.h_reset) copy16(ta.h_reset + e0, t.reset, epb * 8);
-    if (ta.h_timeout) copy16(ta.h_timeout + e0, t.to, epb);
-}
-
 // compute_cartpole_reward, cartpole.py:180-196
 __device__ __forceinline__ void cartpole_reward(float pole_angle, float pole_vel, float cart_vel, float cart_pos,
                                                 float reset_dist, long long progress, float max_len,
