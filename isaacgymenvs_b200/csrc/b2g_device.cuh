@@ -401,14 +401,53 @@ __device__ __forceinline__ bool sphere_box(const float cen[3], float rad, const 
     matvec(Rb, nl, n);
     return true;
 }
-// h * J^T G J of a point contact at r (about O) with G = gam*1 + (gn-gam) n n^T, added to a packed 6x6
-__device__ __forceinline__ void contact_inertia(float IA[21], float h, float gam, float gn, const float r[3], const float n[3]) {
+// the implicit term h J^T G J of a point contact at r (about O), G = gam 1 + (gn - gam) n n^T, added to a packed 6x6;
+// rows of J: j_k = (r x e_k ; e_k).  PLANE: the ground plane z = 0 folded in (n = e_z, not read): G = diag(gam, gam, gn).
+// Every contact of both sub-steps adds its implicit term here.  Fn, gam, F0 and the applied force stay written out at
+// each contact: moved into shared functions they changed which products the compiler fuses into FMAs, and so the
+// results, of some kernels (the four-chain Ant step among them).
+template <bool PLANE>
+B2G_HD void contact_implicit(float IA[21], float h, float gam, float gn, const float r[3], const float n[3]) {
     const float hgam = h * gam;
-    const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
-    const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
-    sym6_rank1(IA, hgam, jx, ex); sym6_rank1(IA, hgam, jy, ey); sym6_rank1(IA, hgam, jz, ez);
-    float rxn[3]; cross(r, n, rxn);
-    sym6_rank1(IA, h * (gn - gam), rxn, n);
+    if (PLANE) {
+        // the same three rank-1 terms with G = diag(gam, gam, gn), zeros folded away
+        const float hgn = h * gn, rx = r[0], ry = r[1], rz = r[2];
+        IA[0] += hgam * rz * rz + hgn * ry * ry;
+        IA[1] += hgam * rz * rz + hgn * rx * rx;
+        IA[2] += hgam * (rx * rx + ry * ry);
+        IA[3] -= hgn * rx * ry; IA[4] -= hgam * rx * rz; IA[5] -= hgam * ry * rz;
+        IA[7] -= hgam * rz; IA[8] += hgn * ry;
+        IA[9] += hgam * rz; IA[11] -= hgn * rx;
+        IA[12] -= hgam * ry; IA[13] += hgam * rx;
+        IA[15] += hgam; IA[16] += hgam; IA[17] += hgn;
+    } else {
+        const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
+        const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
+        sym6_rank1(IA, hgam, jx, ex); sym6_rank1(IA, hgam, jy, ey); sym6_rank1(IA, hgam, jz, ez);
+        float rxn[3]; cross(r, n, rxn);
+        sym6_rank1(IA, h * (gn - gam), rxn, n);
+    }
+}
+// height h and unit normal n of the height field at world (x, y): samples hf[ix * ny + iy] times vscale on a grid of
+// spacing 1 / inv_scale from (ox, oy), each cell split into two triangles
+B2G_HD void hf_sample(const int16_t *hf, int nx, int ny, float inv_scale, float vscale, float ox, float oy,
+                      float x, float y, float &h, float n[3]) {
+    const float fx = (x - ox) * inv_scale, fy = (y - oy) * inv_scale;
+    int ix = (int)floorf(fx), iy = (int)floorf(fy);
+    ix = max(0, min(ix, nx - 2)); iy = max(0, min(iy, ny - 2));
+    const float tx = fminf(fmaxf(fx - ix, 0.f), 1.f), ty = fminf(fmaxf(fy - iy, 0.f), 1.f);
+    const int16_t *p = hf + (size_t)ix * ny + iy;         // height samples: global memory, read-only path
+#ifdef __CUDA_ARCH__
+    const float h00 = __ldg(p) * vscale, h01 = __ldg(p + 1) * vscale, h10 = __ldg(p + ny) * vscale, h11 = __ldg(p + ny + 1) * vscale;
+#else
+    const float h00 = p[0] * vscale, h01 = p[1] * vscale, h10 = p[ny] * vscale, h11 = p[ny + 1] * vscale;
+#endif
+    float dhx, dhy;
+    if (tx + ty <= 1.f) { dhx = h10 - h00; dhy = h01 - h00; h = h00 + tx * dhx + ty * dhy; }
+    else { dhx = h11 - h01; dhy = h11 - h10; h = h11 - (1.f - tx) * dhx - (1.f - ty) * dhy; }
+    const float gx = dhx * inv_scale, gy = dhy * inv_scale;
+    const float inv = b2g_rsqrt(gx * gx + gy * gy + 1.f);
+    n[0] = -gx * inv; n[1] = -gy * inv; n[2] = inv;
 }
 
 struct Ground {
@@ -419,19 +458,7 @@ struct Ground {
     // height and unit normal at world (x, y)
     __device__ __forceinline__ void sample(float x, float y, float &h, float n[3]) const {
         if (!m->has_hf) { h = 0.f; n[0] = 0.f; n[1] = 0.f; n[2] = 1.f; return; }
-        float fx = (x - m->hf_ox) * m->hf_inv_scale, fy = (y - m->hf_oy) * m->hf_inv_scale;
-        int ix = (int)floorf(fx), iy = (int)floorf(fy);
-        ix = max(0, min(ix, m->hf_nx - 2)); iy = max(0, min(iy, m->hf_ny - 2));
-        float tx = fminf(fmaxf(fx - ix, 0.f), 1.f), ty = fminf(fmaxf(fy - iy, 0.f), 1.f);
-        const int16_t *p = hf + (size_t)ix * m->hf_ny + iy;         // height samples: global memory, read-only path
-        float h00 = __ldg(p) * m->hf_vscale, h01 = __ldg(p + 1) * m->hf_vscale;
-        float h10 = __ldg(p + m->hf_ny) * m->hf_vscale, h11 = __ldg(p + m->hf_ny + 1) * m->hf_vscale;
-        float dhx, dhy;
-        if (tx + ty <= 1.f) { dhx = h10 - h00; dhy = h01 - h00; h = h00 + tx * dhx + ty * dhy; }
-        else { dhx = h11 - h01; dhy = h11 - h10; h = h11 - (1.f - tx) * dhx - (1.f - ty) * dhy; }
-        float gx = dhx * m->hf_inv_scale, gy = dhy * m->hf_inv_scale;
-        float inv = rsqrtf(gx * gx + gy * gy + 1.f);
-        n[0] = -gx * inv; n[1] = -gy * inv; n[2] = inv;
+        hf_sample(hf, m->hf_nx, m->hf_ny, m->hf_inv_scale, m->hf_vscale, m->hf_ox, m->hf_oy, x, y, h, n);
     }
 };
 
@@ -486,26 +513,7 @@ __device__ __forceinline__ void link_contacts(const DevModel *m, const Ground &g
             float rxF[3]; cross(r, F0, rxF);
             pa[0] -= rxF[0]; pa[1] -= rxF[1]; pa[2] -= rxF[2];
             pl[0] -= F0[0]; pl[1] -= F0[1]; pl[2] -= F0[2];
-            const float hgam = h * gam;
-            if (HF) {
-                // J^T G J with G = gam*1 + (gn-gam) n n^T ; rows of J: j_k = (r x e_k ; e_k)
-                const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
-                const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
-                sym6_rank1(IA, hgam, jx, ex); sym6_rank1(IA, hgam, jy, ey); sym6_rank1(IA, hgam, jz, ez);
-                float rxn[3]; cross(r, n, rxn);
-                sym6_rank1(IA, h * (gn - gam), rxn, n);
-            } else {
-                // the same three rank-1 terms with G = diag(gam, gam, gn), zeros folded away
-                const float hgn = h * gn, rx = r[0], ry = r[1], rz = r[2];
-                IA[0] += hgam * rz * rz + hgn * ry * ry;
-                IA[1] += hgam * rz * rz + hgn * rx * rx;
-                IA[2] += hgam * (rx * rx + ry * ry);
-                IA[3] -= hgn * rx * ry; IA[4] -= hgam * rx * rz; IA[5] -= hgam * ry * rz;
-                IA[7] -= hgam * rz; IA[8] += hgn * ry;
-                IA[9] += hgam * rz; IA[11] -= hgn * rx;
-                IA[12] -= hgam * ry; IA[13] += hgam * rx;
-                IA[15] += hgam; IA[16] += hgam; IA[17] += hgn;
-            }
+            contact_implicit<!HF>(IA, h, gam, gn, r, n);
         } else {
             float axr[3]; cross(aw, r, axr);
             const float Ja[3] = {al[0] + axr[0], al[1] + axr[1], al[2] + axr[2]};
@@ -730,7 +738,7 @@ struct Stepper {
         const float gam = smu * Fn * rsqrtf(dot3(ut, ut) + m->vs2);
         const float F0[3] = {Fn * n_[0] - gam * ut[0], Fn * n_[1] - gam * ut[1], Fn * n_[2] - gam * ut[2]};
         if (ACCUM) {
-            contact_inertia(IA, h, gam, gn, r, n_);
+            contact_implicit<false>(IA, h, gam, gn, r, n_);
             float rxF[3]; cross(r, F0, rxF);
 #pragma unroll
             for (int c = 0; c < 3; c++) { pa[c] -= rxF[c]; pl[c] -= F0[c]; }
@@ -952,7 +960,7 @@ struct Stepper {
             float dM[21];
 #pragma unroll
             for (int c = 0; c < 21; c++) dM[c] = 0.f;
-            contact_inertia(dM, h, gam, gn, r, n);
+            contact_implicit<false>(dM, h, gam, gn, r, n);
             float rxF[3]; cross(r, F0, rxF);
 #pragma unroll
             for (int c = 0; c < 21; c++) IA[c] += dM[c];
@@ -1067,7 +1075,7 @@ struct Stepper {
             if (Fn <= 0.f) continue;
             const float gam = op.w * Fn * rsqrtf(u[0] * u[0] + u[1] * u[1] + m->vs2);
             const float F0[3] = {-gam * u[0], -gam * u[1], Fn}, ez[3] = {0.f, 0.f, 1.f};
-            contact_inertia(Io, h, gam, gn, r, ez);
+            contact_implicit<false>(Io, h, gam, gn, r, ez);
             float rxF[3]; cross(r, F0, rxF);
 #pragma unroll
             for (int c = 0; c < 3; c++) { pao[c] -= rxF[c]; plo[c] -= F0[c]; }

@@ -116,23 +116,7 @@ struct QLane {
     B2G_HD void ground(float x, float y, float &hgt, float n[3]) const {
         if (!HF) { hgt = 0.f; n[0] = 0.f; n[1] = 0.f; n[2] = 1.f; return; }
         const float4 H2 = qm[2], H3 = qm[3];
-        const int nx = q_f2i(H3.x), ny = q_f2i(H3.y);
-        const float fx = (x - H2.z) * H2.x, fy = (y - H2.w) * H2.x;
-        int ix = (int)floorf(fx), iy = (int)floorf(fy);
-        ix = max(0, min(ix, nx - 2)); iy = max(0, min(iy, ny - 2));
-        const float tx = fminf(fmaxf(fx - ix, 0.f), 1.f), ty = fminf(fmaxf(fy - iy, 0.f), 1.f);
-        const int16_t *p = hf + (size_t)ix * ny + iy;
-#ifdef __CUDA_ARCH__
-        const float h00 = __ldg(p) * H2.y, h01 = __ldg(p + 1) * H2.y, h10 = __ldg(p + ny) * H2.y, h11 = __ldg(p + ny + 1) * H2.y;
-#else
-        const float h00 = p[0] * H2.y, h01 = p[1] * H2.y, h10 = p[ny] * H2.y, h11 = p[ny + 1] * H2.y;
-#endif
-        float dhx, dhy;
-        if (tx + ty <= 1.f) { dhx = h10 - h00; dhy = h01 - h00; hgt = h00 + tx * dhx + ty * dhy; }
-        else { dhx = h11 - h01; dhy = h11 - h10; hgt = h11 - (1.f - tx) * dhx - (1.f - ty) * dhy; }
-        const float gx = dhx * H2.x, gy = dhy * H2.x;
-        const float inv = q_rsqrt(gx * gx + gy * gy + 1.f);
-        n[0] = -gx * inv; n[1] = -gy * inv; n[2] = inv;
+        hf_sample(hf, q_f2i(H3.x), q_f2i(H3.y), H2.x, H2.y, H2.z, H2.w, x, y, hgt, n);
     }
 
     // ---- one contact sphere (link-frame centre cp.xyz, radius cp.w) of a link posed at (R, x) with twist (vw, vl).
@@ -182,24 +166,7 @@ struct QLane {
         if (ACCUM) {
             cross_sub<FACC>(r, F0, pa);
             pl[0] -= F0[0]; pl[1] -= F0[1]; pl[2] -= F0[2];
-            const float hgam = h * gam;
-            if (HF) {
-                const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
-                const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
-                sym6_rank1(I, hgam, jx, ex); sym6_rank1(I, hgam, jy, ey); sym6_rank1(I, hgam, jz, ez);
-                float rxn[3]; cross(r, n, rxn);
-                sym6_rank1(I, h * (gn - gam), rxn, n);
-            } else {
-                const float hgn = h * gn, rx = r[0], ry = r[1], rz = r[2];
-                I[0] += hgam * rz * rz + hgn * ry * ry;
-                I[1] += hgam * rz * rz + hgn * rx * rx;
-                I[2] += hgam * (rx * rx + ry * ry);
-                I[3] -= hgn * rx * ry; I[4] -= hgam * rx * rz; I[5] -= hgam * ry * rz;
-                I[7] -= hgam * rz; I[8] += hgn * ry;
-                I[9] += hgam * rz; I[11] -= hgn * rx;
-                I[12] -= hgam * ry; I[13] += hgam * rx;
-                I[15] += hgam; I[16] += hgam; I[17] += hgn;
-            }
+            contact_implicit<!HF>(I, h, gam, gn, r, n);
         } else {
             float Ja[3]; cross_add(aw, r, al, Ja);
             float Fk[3];
@@ -363,12 +330,7 @@ struct QLane {
         if (ACCUM) {
             cross_sub<FACC>(r, F0, pa);
             pl[0] -= F0[0]; pl[1] -= F0[1]; pl[2] -= F0[2];
-            const float hgam = h * gam;
-            const float jx[3] = {0.f, r[2], -r[1]}, jy[3] = {-r[2], 0.f, r[0]}, jz[3] = {r[1], -r[0], 0.f};
-            const float ex[3] = {1.f, 0.f, 0.f}, ey[3] = {0.f, 1.f, 0.f}, ez[3] = {0.f, 0.f, 1.f};
-            sym6_rank1(I, hgam, jx, ex); sym6_rank1(I, hgam, jy, ey); sym6_rank1(I, hgam, jz, ez);
-            float rxn[3]; cross(r, n, rxn);
-            sym6_rank1(I, h * (gn - gam), rxn, n);
+            contact_implicit<false>(I, h, gam, gn, r, n);
         } else {
             float Ja[3]; cross_add(aw, r, al, Ja);
             const float Jan = dot3(Ja, n);
